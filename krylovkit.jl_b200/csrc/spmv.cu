@@ -59,6 +59,15 @@ struct b2k_op {
 
 namespace {
 
+// Products and sums rounded on their own: with nvcc's default -fmad=true, `acc += (double)(a * b)` is one DFMA for
+// T = double (the cast is a no-op), so the product would not be rounded before it is added.
+template <typename T> __device__ __forceinline__ T mul_rn(T a, T b);
+template <> __device__ __forceinline__ double mul_rn<double>(double a, double b) { return __dmul_rn(a, b); }
+template <> __device__ __forceinline__ float mul_rn<float>(float a, float b) { return __fmul_rn(a, b); }
+template <typename T> __device__ __forceinline__ T add_rn(T a, T b);
+template <> __device__ __forceinline__ double add_rn<double>(double a, double b) { return __dadd_rn(a, b); }
+template <> __device__ __forceinline__ float add_rn<float>(float a, float b) { return __fadd_rn(a, b); }
+
 template <typename T>
 __global__ void __launch_bounds__(SP_BT)
 k_spmv_stream(const int32_t* __restrict__ rowptr, const int32_t* __restrict__ colidx,
@@ -136,7 +145,7 @@ k_spmv_stream(const int32_t* __restrict__ rowptr, const int32_t* __restrict__ co
             const int32_t cc = colidx[p0 + i];
             T xv = (cc < n_loc) ? __ldg(x + cc) : __ldg(halo + (cc - n_loc));
             if (scaled) xv *= sc;
-            acc += (double)(vals[p0 + i] * xv);
+            acc += (double)mul_rn<T>(vals[p0 + i], xv);
         }
         const double tot = block_sum(acc, red);
         if (tid == 0) {
@@ -357,7 +366,7 @@ k_spmv_pipe(const int32_t* __restrict__ rowptr, const int32_t* __restrict__ coli
                 const int32_t cc = colidx[p0 + i];
                 T xv = (cc < n_loc) ? __ldg(x + cc) : __ldg(halo + (cc - n_loc));
                 if (scaled) xv *= sc;
-                acc += (double)(vals[p0 + i] * xv);
+                acc += (double)mul_rn<T>(vals[p0 + i], xv);
             }
             acc = warp_sum(acc);
             if (lane == 0) red[w] = acc;
@@ -434,13 +443,6 @@ constexpr int SPM_PMAX = 8;
 struct SpmmCols {
     int32_t x[SPM_PMAX], y[SPM_PMAX];
 };
-
-template <typename T> __device__ __forceinline__ T mul_rn(T a, T b);
-template <> __device__ __forceinline__ double mul_rn<double>(double a, double b) { return __dmul_rn(a, b); }
-template <> __device__ __forceinline__ float mul_rn<float>(float a, float b) { return __fmul_rn(a, b); }
-template <typename T> __device__ __forceinline__ T add_rn(T a, T b);
-template <> __device__ __forceinline__ double add_rn<double>(double a, double b) { return __dadd_rn(a, b); }
-template <> __device__ __forceinline__ float add_rn<float>(float a, float b) { return __fadd_rn(a, b); }
 
 template <typename T>
 __global__ void __launch_bounds__(SPP_THREADS, 3)
