@@ -700,7 +700,7 @@ extern "C" int32_t b2k_block_orthogonalize(b2k_ctx* ctx, const b2k_vec* Rb, int3
 // Flagged block_qr! (blocklanczos.jl:312-353): CholeskyQR2.  G = X' X (one pass), G = L L' on the host,
 // X <- X L^-T (triangular basis transform, in place), twice; R = L2' L1' is upper triangular with a positive
 // diagonal, i.e. the SAME factor modified Gram-Schmidt produces (the QR factorization with positive diagonal is
-// unique), to rounding.  *ok = 0 when a Cholesky pivot falls below (100 tol)^2 relative to its column's norm^2
+// unique), to rounding.  *ok = 0 when a Cholesky pivot falls below (100 tol)^2 or 9e4 u times its column's norm^2
 // (numerically rank-deficient block: the caller falls back to the reference's MGS b2k_block_qr, which knows how
 // to drop vectors); X is then unchanged.
 extern "C" int32_t b2k_block_cholqr(b2k_ctx* ctx, const b2k_vec* X, int32_t p, double tol, const double* G0_host,
@@ -712,6 +712,14 @@ extern "C" int32_t b2k_block_cholqr(b2k_ctx* ctx, const b2k_vec* X, int32_t p, d
     double* d_G = ctx->d_blk + 2 * HCAP;
     std::vector<double> G(p * p), L(p * p), Rtot(p * p, 0.0), Linv(p * p);
     for (int i = 0; i < p; ++i) Rtot[i * p + i] = 1.0;
+    // A Cholesky pivot is ||x_j - proj||^2 formed by SUBTRACTION: it carries an absolute error of ~u ||x_j||^2, with
+    // u the unit roundoff of the vector type (the Gram matrix is accumulated from products rounded in T), so
+    // CholeskyQR can neither resolve a residual below sqrt(u) ||x_j|| nor orthogonalise a block with condition number
+    // above ~u^-1/2.  Accept only pivots well above that noise: relative 9e4 u, i.e. 1e-11 in Float64 (kappa < 3e5 —
+    // the second round then restores orthogonality to eps) and 5.4e-3 in Float32 (kappa < 14; a Float32 pivot of
+    // relative 1e-11 is noise, and the second Cholesky of such a block can fail) — AND above block_qr!'s own absolute
+    // scale (100 tol)^2; everything else goes to the reference MGS path.
+    const double rel_pivot = 1e-11 * (ctx->dtype == B2K_F64 ? 1.0 : 0x1p-24 / 0x1p-53);
     for (int round = 0; round < 2; ++round) {
         if (round == 0 && G0_host) {
             memcpy(G.data(), G0_host, sizeof(double) * p * p);
@@ -724,12 +732,7 @@ extern "C" int32_t b2k_block_cholqr(b2k_ctx* ctx, const b2k_vec* X, int32_t p, d
         for (int j = 0; j < p; ++j) {
             double d = G[j * p + j];
             for (int t = 0; t < j; ++t) d -= L[t * p + j] * L[t * p + j];
-            // A Cholesky pivot is ||x_j - proj||^2 formed by SUBTRACTION: it carries an absolute error of
-            // ~eps ||x_j||^2, so CholeskyQR can neither resolve a residual below sqrt(eps) ||x_j|| nor
-            // orthogonalise a block with condition number above ~eps^-1/2.  Accept only pivots well above that
-            // noise (relative 1e-11, i.e. kappa < 3e5 — the second round then restores orthogonality to eps) AND
-            // above block_qr!'s own absolute scale (100 tol)^2; everything else goes to the reference MGS path.
-            const double thr = (round == 0) ? std::max((100.0 * tol) * (100.0 * tol), 1e-11 * G[j * p + j]) : 0.0;
+            const double thr = (round == 0) ? std::max((100.0 * tol) * (100.0 * tol), rel_pivot * G[j * p + j]) : 0.0;
             if (!(d > thr) || !(d > 1e-28 * G[j * p + j])) {
                 if (round == 0) return B2K_OK;             // *ok = 0, X untouched
                 return b2k_fail(ctx, B2K_ECUDA, "block_cholqr: second Cholesky lost positivity");

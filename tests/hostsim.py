@@ -789,6 +789,7 @@ class HostSimLib:
         sh = self._sh(ctx, list(X)[0])
         Xs = np.column_stack([self._vec(ctx, c).astype(np.float64) for c in list(X)[:p]])
         Rtot = np.eye(p)
+        rel = 1e-11 * (np.finfo(ctx.dtype).eps / np.finfo(np.float64).eps)    # block.cu: 9e4 u of the vector type
         _set(ok, 0)
         for rnd in range(2):
             G = np.array([[ctx.allsum(np.dot(Xs[:, i], Xs[:, j]), sh)[0] for j in range(p)] for i in range(p)])
@@ -796,7 +797,7 @@ class HostSimLib:
                 Lc = np.linalg.cholesky(G)
             except np.linalg.LinAlgError:
                 return L.OK
-            if rnd == 0 and np.any(np.diag(Lc) ** 2 <= np.maximum((100 * tol) ** 2, 1e-11 * np.diag(G))):
+            if rnd == 0 and np.any(np.diag(Lc) ** 2 <= np.maximum((100 * tol) ** 2, rel * np.diag(G))):
                 return L.OK
             Xs = np.linalg.solve(Lc, Xs.T).T
             Rtot = Lc.T @ Rtot
