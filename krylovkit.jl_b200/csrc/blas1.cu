@@ -123,7 +123,10 @@ __global__ void __launch_bounds__(BT) k_scale(T* __restrict__ y, const T* __rest
 }
 
 // y = beta*y + alpha*x   (beta == 0 never reads y: hard zero semantics)
-template <typename T, int MODE>   // MODE 0: beta==0, 1: beta==1, 2: general
+// Rounding: MODE 0 rn(alpha*x), MODE 1 fma(alpha, x, y), MODE 2 fma(alpha, x, rn(beta*y)).
+// SELF (add!!(y, y, alpha, beta)): x is y, read once through y (x is not dereferenced), with the same rounding as a
+// call on a copy of y — not rn((alpha + beta) * y), which differs in the last bit for most entries.
+template <typename T, int MODE, bool SELF>   // MODE 0: beta==0, 1: beta==1, 2: general
 __global__ void __launch_bounds__(BT) k_axpby(T* __restrict__ y, const T* __restrict__ x,
                                               int64_t n, T alpha, T beta) {
     constexpr int V = Vec16<T>::N;
@@ -132,24 +135,26 @@ __global__ void __launch_bounds__(BT) k_axpby(T* __restrict__ y, const T* __rest
     B2K_TRIP(4) {
         T a[4][V], b[4][V];
         B2K_EACH(4, u, i) {
-            vload<T>(x + i * V, a[u]);
-            if (MODE != 0) vload<T>(y + i * V, b[u]);
+            if (!SELF) vload<T>(x + i * V, a[u]);
+            if (SELF || MODE != 0) vload<T>(y + i * V, b[u]);
         }
         B2K_EACH(4, u, i) {
 #pragma unroll
             for (int j = 0; j < V; ++j) {
-                if (MODE == 0) b[u][j] = alpha * a[u][j];
-                else if (MODE == 1) b[u][j] = fma(alpha, a[u][j], b[u][j]);
-                else b[u][j] = fma(alpha, a[u][j], beta * b[u][j]);
+                const T xv = SELF ? b[u][j] : a[u][j];
+                if (MODE == 0) b[u][j] = alpha * xv;
+                else if (MODE == 1) b[u][j] = fma(alpha, xv, b[u][j]);
+                else b[u][j] = fma(alpha, xv, beta * b[u][j]);
             }
             vstore<T>(y + i * V, b[u]);
         }
     }
     if (blockIdx.x == 0 && threadIdx.x < (n - nv * V)) {
         int64_t i = nv * V + threadIdx.x;
-        if (MODE == 0) y[i] = alpha * x[i];
-        else if (MODE == 1) y[i] = fma(alpha, x[i], y[i]);
-        else y[i] = fma(alpha, x[i], beta * y[i]);
+        const T xv = SELF ? y[i] : x[i];
+        if (MODE == 0) y[i] = alpha * xv;
+        else if (MODE == 1) y[i] = fma(alpha, xv, y[i]);
+        else y[i] = fma(alpha, xv, beta * y[i]);
     }
 }
 
@@ -179,7 +184,20 @@ __global__ void __launch_bounds__(BT) k_axpy2(T* __restrict__ y, const T* __rest
     }
 }
 
+__device__ __forceinline__ double mul_rn(double a, double b) { return __dmul_rn(a, b); }
+__device__ __forceinline__ float mul_rn(float a, float b) { return __fmul_rn(a, b); }
+
 // (q1,q2) <- (c*q1 - s*q2, s*q1 + c*q2)   — dense/givens.jl:22-36
+// Rounded as rmul!(b, G) does it for a vector type with add / add!! (givens.jl:30-36):
+//   q1' = add(q1, q2, -s, c)   = fma(-s, q2, rn(c*q1))
+//   q2' = add!!(q2, q1, s, c)  = fma(s, q1, rn(c*q2))
+// The pairing is spelled out with fma and an explicitly rounded product, so nvcc's contraction has no choice to make.
+template <typename T>
+__device__ __forceinline__ void givens_rn(T c, T s, T a, T b, T& o1, T& o2) {
+    o1 = fma(-s, b, mul_rn(c, a));
+    o2 = fma(s, a, mul_rn(c, b));
+}
+
 template <typename T>
 __global__ void __launch_bounds__(BT) k_givens(T* __restrict__ q1, T* __restrict__ q2, int64_t n,
                                                T c, T s) {
@@ -195,19 +213,17 @@ __global__ void __launch_bounds__(BT) k_givens(T* __restrict__ q1, T* __restrict
         B2K_EACH(4, u, i) {
             T o1[V], o2[V];
 #pragma unroll
-            for (int j = 0; j < V; ++j) {
-                o1[j] = c * a[u][j] - s * b[u][j];
-                o2[j] = s * a[u][j] + c * b[u][j];
-            }
+            for (int j = 0; j < V; ++j) givens_rn(c, s, a[u][j], b[u][j], o1[j], o2[j]);
             vstore<T>(q1 + i * V, o1);
             vstore<T>(q2 + i * V, o2);
         }
     }
     if (blockIdx.x == 0 && threadIdx.x < (n - nv * V)) {
         int64_t i = nv * V + threadIdx.x;
-        T a = q1[i], b = q2[i];
-        q1[i] = c * a - s * b;
-        q2[i] = s * a + c * b;
+        T o1, o2;
+        givens_rn(c, s, q1[i], q2[i], o1, o2);
+        q1[i] = o1;
+        q2[i] = o2;
     }
 }
 
@@ -705,13 +721,17 @@ extern "C" int32_t b2k_vec_axpby(b2k_ctx* ctx, b2k_vec y, b2k_vec x, double alph
     B2K_TRY(b2k_resolve(ctx, x, &rx));
     if (ry.n != rx.n) return b2k_fail(ctx, B2K_EDIM, "vec_axpby: length mismatch");
     if (ry.n == 0) return B2K_OK;
-    if (ry.ptr == rx.ptr) {   // y <- (beta + alpha) * y would change rounding; do it literally
-        return b2k_vec_scale(ctx, y, x, beta + alpha);
-    }
+    // add!!(y, y, alpha, beta): y <- (beta + alpha) * y would change rounding; do it literally, reading y once
+    const bool self = ry.ptr == rx.ptr;
     const int grid = grid_for(ctx, ry.n, 8);
-#define LAUNCH(T, MODE)                                                                    \
-    k_axpby<T, MODE><<<grid, BT, 0, ctx->stream>>>((T*)ry.ptr, (const T*)rx.ptr, ry.n,     \
-                                                   (T)alpha, (T)beta)
+#define LAUNCH_S(T, MODE, SELF)                                                                              \
+    k_axpby<T, MODE, SELF><<<grid, BT, 0, ctx->stream>>>((T*)ry.ptr, SELF ? nullptr : (const T*)rx.ptr, ry.n, \
+                                                         (T)alpha, (T)beta)
+#define LAUNCH(T, MODE)                       \
+    do {                                      \
+        if (self) LAUNCH_S(T, MODE, true);    \
+        else LAUNCH_S(T, MODE, false);        \
+    } while (0)
     if (ctx->dtype == B2K_F64) {
         if (beta == 0.0) LAUNCH(double, 0);
         else if (beta == 1.0) LAUNCH(double, 1);
@@ -722,6 +742,7 @@ extern "C" int32_t b2k_vec_axpby(b2k_ctx* ctx, b2k_vec y, b2k_vec x, double alph
         else LAUNCH(float, 2);
     }
 #undef LAUNCH
+#undef LAUNCH_S
     B2K_LAUNCH_CHECK(ctx);
     return B2K_OK;
 }
@@ -835,7 +856,7 @@ extern "C" int32_t b2k_vec_orthogonalize(b2k_ctx* ctx, b2k_vec v, b2k_vec q, int
         double nold = sqrt(ctx->h_res[1]);
         s = ctx->h_res[0];
         double nnew = sqrt(ctx->h_res[2]);
-        const double eps = (ctx->dtype == B2K_F64) ? 2.220446049250313e-16 : 1.1920929e-07;
+        const double eps = (ctx->dtype == B2K_F64) ? 0x1p-52 : 0x1p-23;    // eps(T), orthonormal.jl:481
         while (eps < nnew && nnew < eta * nold) {
             nold = nnew;
             B2K_TRY(dot(0));
