@@ -144,6 +144,7 @@ _PROTOS = {
     "b2k_debug_set_spmv_variant": (C.c_int32, [C.c_int32]),
     "b2k_debug_set_dmma": (C.c_int32, [C.c_int32]),
     "b2k_debug_set_transform": (C.c_int32, [C.c_int32]),
+    "b2k_debug_transform_kernel": (C.c_int32, []),
     "b2k_debug_set_chain": (C.c_int32, [C.c_int32]),
     "b2k_debug_used_columns": (C.c_int32, [c_ctx, C.c_int32]),
     "b2k_debug_set_chain_mode": (C.c_int32, [C.c_int32]),

@@ -1289,6 +1289,11 @@ bool g_use_dmma = true;
 int g_transform_ur = 0;      // B2K_TRANSFORM_UR: 0 = DMMA kernel, 1 = <2 rows x 18>, 2 = <2 x 36>, 3 = <4 x 18> (DFMA, U in the constant bank)
 int g_transform_hyb = 2;     // B2K_TRANSFORM_HYB: 2 (default) = DFMA 8 x 9 tile for keep <= 36 (k_transform_f89),
                              // 0 = DMMA kernel, 1 = DMMA + DFMA hybrid (k_transform_hyb)
+// the restart-GEMM kernel the last b2k_basis_transform launched (b2k_debug_transform_kernel): 0 = none yet,
+// 1 / 2 = k_transform<double, U in smem / global>, 3 / 4 = k_transform<float, smem / global>,
+// 5 / 6 = k_transform_big<double / float>, 7 / 8 / 9 = k_transform_ur<2,18> / <2,36> / <4,18>,
+// 10 = k_transform_f89, 11 = k_transform_f89w, 12 = k_transform_hyb, 13 = k_transform_dmma
+int g_transform_kernel = 0;
 
 // modified Gram-Schmidt sweep, pipelined: launch j computes v -= s_{j-1} q_{j-1} and
 // s_j = <q_j, v> in one pass (orthonormal.jl:417-421).  d_res[res_off + j] = s_j;
@@ -1389,6 +1394,9 @@ extern "C" int32_t b2k_debug_set_transform(int32_t mode) {
     g_transform_hyb = mode == 4 ? 1 : (mode == 5 ? 2 : (mode == 7 ? 3 : (mode == 0 ? 2 : 0)));   // 0 = default, 4 = hybrid, 5 = 8 x 9 (two sets, alternate tiles), 6 = DMMA, 7 = 8 x 9 on 512-row tiles
     return B2K_OK;
 }
+
+// which kernel the last b2k_basis_transform launched (ids at g_transform_kernel): tests assert the dispatch with it
+extern "C" int32_t b2k_debug_transform_kernel(void) { return g_transform_kernel; }
 
 extern "C" int32_t b2k_debug_set_coop(int32_t on) {
     g_use_coop = on != 0;
@@ -2068,6 +2076,14 @@ extern "C" int32_t b2k_basis_transform(b2k_ctx* ctx, const b2k_vec* cols, int32_
     if (!ctx || !cols || !U_host || m < 1 || keep < 1 || keep > m || ldu < m) return B2K_EINVAL;
     Panel pn;
     B2K_TRY(make_panel(ctx, cols, m, &pn));
+    {   // a column listed twice would be two outputs in one storage, written by different threads
+        std::vector<uint8_t> seen(ctx->spaces[B2K_VEC_SPACE(cols[0])].ncols, 0);
+        for (int i = 0; i < m; ++i) {
+            if (seen[pn.idx[i]])
+                return b2k_fail(ctx, B2K_EINVAL, "basis_transform: column %d is listed twice", pn.idx[i]);
+            seen[pn.idx[i]] = 1;
+        }
+    }
     const bool f64 = ctx->dtype == B2K_F64;
     const int C = f64 ? 8 : 16;
     if (m > 256)
@@ -2097,6 +2113,7 @@ extern "C" int32_t b2k_basis_transform(b2k_ctx* ctx, const b2k_vec* cols, int32_
         const size_t smem = (size_t)TB_ROWS * m * ctx->esize;
         const int per_sm = (int)std::max<size_t>(1, std::min<size_t>(4, (size_t)(200 * 1024) / smem));
         const int grid = (int)std::min<int64_t>(ntiles, (int64_t)ctx->num_sms * per_sm);
+        g_transform_kernel = f64 ? 5 : 6;
         if (f64) k_transform_big<double><<<grid, TB_THREADS, smem, ctx->stream>>>(p, cl);
         else k_transform_big<float><<<grid, TB_THREADS, smem, ctx->stream>>>(p, cl);
     } else if (f64 && g_transform_ur && keep <= UR_J && m <= UR_MAXM) {
@@ -2105,24 +2122,31 @@ extern "C" int32_t b2k_basis_transform(b2k_ctx* ctx, const b2k_vec* cols, int32_
         for (int j = 0; j < keep; ++j)
             for (int i = 0; i < m; ++i) up.u[i * UR_J + j] = U_host[(size_t)j * ldu + i];
         const int grid = grid_for_rows<double>(ctx, pn.n);
+        g_transform_kernel = 6 + g_transform_ur;
         if (g_transform_ur == 1) k_transform_ur<2, 18><<<grid, TR_THREADS, TR_SMEM, ctx->stream>>>(p, cl, up);
         else if (g_transform_ur == 2) k_transform_ur<2, 36><<<grid, TR_THREADS, TR_SMEM, ctx->stream>>>(p, cl, up);
         else k_transform_ur<4, 18><<<grid, TR_THREADS, TR_SMEM, ctx->stream>>>(p, cl, up);
     } else if (f64 && g_transform_hyb == 3 && keep <= F89_G * F89_TH &&
                (size_t)F89_G * m * F89_UP * 8 <= (size_t)TR_U_BYTES - 64) {
         const int64_t nt = (pn.n + F89W_R - 1) / F89W_R;
+        g_transform_kernel = 11;
         k_transform_f89w<<<(int)std::max<int64_t>(1, std::min<int64_t>(nt, ctx->num_sms)), F89_THREADS, TR_SMEM, ctx->stream>>>(p, cl);
     } else if (f64 && g_transform_hyb == 2 && keep <= F89_G * F89_TH &&
                (size_t)F89_G * m * F89_UP * 8 <= (size_t)TR_U_BYTES - 64) {
+        g_transform_kernel = 10;
         k_transform_f89<<<grid_for_rows<double>(ctx, pn.n), F89_THREADS, TR_SMEM, ctx->stream>>>(p, cl);
     } else if (dmma_ok && g_transform_hyb == 1 && keep <= TH_MAXKEEP && (size_t)m * 40 * 8 <= (size_t)TD_U_BYTES) {
+        g_transform_kernel = 12;
         k_transform_hyb<<<grid_for_rows<double>(ctx, pn.n), TR_THREADS, TD_SMEM, ctx->stream>>>(p, cl);
     } else if (dmma_ok) {
+        g_transform_kernel = 13;
         k_transform_dmma<<<grid_for_rows<double>(ctx, pn.n), TR_THREADS, TD_SMEM, ctx->stream>>>(p, cl);
     } else if (f64) {
+        g_transform_kernel = p.u_in_smem ? 1 : 2;
         if (p.u_in_smem) k_transform<double, true><<<grid_for_rows<double>(ctx, pn.n), TR_THREADS, TR_SMEM, ctx->stream>>>(p, cl);
         else k_transform<double, false><<<grid_for_rows<double>(ctx, pn.n), TR_THREADS, TR_SMEM, ctx->stream>>>(p, cl);
     } else {
+        g_transform_kernel = p.u_in_smem ? 3 : 4;
         if (p.u_in_smem) k_transform<float, true><<<grid_for_rows<float>(ctx, pn.n), TR_THREADS, TR_SMEM, ctx->stream>>>(p, cl);
         else k_transform<float, false><<<grid_for_rows<float>(ctx, pn.n), TR_THREADS, TR_SMEM, ctx->stream>>>(p, cl);
     }

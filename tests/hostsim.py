@@ -519,6 +519,16 @@ class HostSimLib:
 
     def b2k_basis_transform(self, h, cols, m, U, ldu, keep):
         ctx = self._c(h)
+        if m < 1 or keep < 1 or keep > m or ldu < m:
+            return L.EINVAL
+        hs = [int(c) for c in list(cols)[:m]]
+        for c in hs:
+            if c < 0 or (c >> 20) >= len(ctx.spaces) or (c & 0xFFFFF) not in ctx.spaces[c >> 20].cols:
+                return self._fail(ctx, L.EINVAL, f"invalid vector handle {c:#x}")
+        if len({c >> 20 for c in hs}) > 1:
+            return self._fail(ctx, L.EDIM, "basis vectors live in different spaces")
+        if len(set(hs)) < m:
+            return self._fail(ctx, L.EINVAL, "basis_transform: a column is listed twice")
         if m > 256:
             return self._fail(ctx, L.ENOTSUP, "basis_transform: m exceeds the supported basis width (256)")
         Um = np.array(_view(U, ldu * keep, C.c_double)).reshape(keep, ldu).T[:m, :]

@@ -8,8 +8,11 @@ pytestmark = pytest.mark.gpu
 
 import krylovkit_jl_b200 as kk
 from krylovkit_jl_b200 import _lib as L
+import test_gpu_transform as T
+from test_gpu_transform import expected_kernel
 
 SEED = 20260923
+UR_KERNEL = {1: T.K_UR218, 2: T.K_UR236, 3: T.K_UR418}
 
 
 def splitmix_host(seed, n, offset=0):
@@ -257,6 +260,7 @@ def test_basistransform(n, m, keep, dtype):
     b = kk.OrthonormalBasis(vecs)
     U, _ = np.linalg.qr(rng.standard_normal((m, m)))
     kk.basistransform_(b, U[:, :keep])
+    assert L.load().b2k_debug_transform_kernel() == expected_kernel(dtype, m, keep)
     ref = Q.astype(np.float64) @ U[:, :keep]
     tol = 1e-12 if dtype == np.float64 else 2e-6
     for j in range(keep):
@@ -286,6 +290,7 @@ def test_basistransform_constant_bank_variants(n, m, keep, mode):
                 v.upload(Q[:, j])
             b = kk.OrthonormalBasis(vecs)
             kk.basistransform_(b, U[:, :keep])
+            assert lib.b2k_debug_transform_kernel() == expected_kernel(np.float64, m, keep, md) == UR_KERNEL[md]
             out = np.column_stack([b[j].to_host() for j in range(m)])
             np.testing.assert_allclose(out[:, :keep], ref, rtol=1e-12, atol=1e-12)
             np.testing.assert_array_equal(out[:, keep:], Q[:, keep:])
@@ -297,12 +302,15 @@ def test_basistransform_constant_bank_variants(n, m, keep, mode):
 
 
 @pytest.mark.parametrize("n,m,keep", [(70001, 60, 36), (5000, 30, 18), (257, 61, 35), (100003, 96, 36), (999, 5, 1),
-                                      (4096, 40, 25), (3001, 59, 31), (777, 36, 36)])
+                                      (4096, 40, 25), (3001, 59, 31), (777, 36, 36),
+                                      # the hybrid at its limit (m <= 92); DMMA at its limit (m·ceil8(keep) = 3680)
+                                      (100003, 92, 36), (20011, 92, 40)])
 @pytest.mark.parametrize("mode", [4, 5, 6, 7], ids=["dmma+dfma", "dfma8x9", "dmma", "dfma8x9-512"])
 def test_basistransform_hybrid_dmma_dfma(n, m, keep, mode):
     """k_transform_hyb (output columns [0, 24) on the FP64 tensor pipe, [24, 36) as register-blocked DFMA, in the same
     warps) and k_transform_f89 (DFMA only, thread <-> 8 rows x 9 outputs) against the dense product, ragged tiles and
-    chunk tails included."""
+    chunk tails included.  At m = 96 neither the hybrid (m·40·8 > 29 440 bytes) nor DMMA (96·40 > 3680) fits: modes 4
+    and 6 fall back to k_transform.  keep = 40 is past every keep <= 36 kernel: all four modes run DMMA."""
     lib = L.load()
     rng = np.random.default_rng(7 * n + m)
     Q, _ = np.linalg.qr(rng.standard_normal((n, m)))
@@ -316,6 +324,14 @@ def test_basistransform_hybrid_dmma_dfma(n, m, keep, mode):
             v.upload(Q[:, j])
         b = kk.OrthonormalBasis(vecs)
         kk.basistransform_(b, U[:, :keep])
+        kid = lib.b2k_debug_transform_kernel()
+        assert kid == expected_kernel(np.float64, m, keep, mode)
+        if m == 96 and mode in (4, 6):
+            assert kid == T.K_F64_SMEM
+        elif keep == 40:
+            assert kid == T.K_DMMA
+        else:
+            assert kid == {4: T.K_HYB, 5: T.K_F89, 6: T.K_DMMA, 7: T.K_F89W}[mode]
         out = np.column_stack([b[j].to_host() for j in range(m)])
         np.testing.assert_allclose(out[:, :keep], ref, rtol=1e-12, atol=1e-12)
         np.testing.assert_array_equal(out[:, keep:], Q[:, keep:])

@@ -250,6 +250,13 @@ def test_bicgstab_chain_bookkeeping(simf):
     G.test_bicgstab_chained_iterations_equal_stepwise()
 
 
+def test_basistransform_refusals(sim):
+    """b2k_basis_transform's refusals (bad sizes, m > 256, two spaces, a repeated handle) leave every column as it
+    was, on the simulator as on the device"""
+    import test_gpu_transform as T
+    T.test_refusals_leave_every_column_untouched(check_kernel=False)
+
+
 def test_block_fast_mode(sim):
     """the flagged block mode's host logic (BCGS2 coefficients -> M, Gram -> CholeskyQR2, rank fallback)"""
     import test_gpu_primitives as P
