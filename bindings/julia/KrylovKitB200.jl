@@ -164,7 +164,9 @@ end
 mutable struct B200CSR{T}
     ctx::B200Ctx
     h::Ptr{Cvoid}
+    adj::Any                              # A' (a B200CSR), built on the device by the first apply_adjoint
 end
+B200CSR{T}(ctx::B200Ctx, h::Ptr{Cvoid}) where {T} = B200CSR{T}(ctx, h, nothing)
 function B200CSR(ctx::B200Ctx, A::SparseMatrixCSC{T, Int64}) where {T}      # colptr / rowval / nzval as stored
     h = Ref{Ptr{Cvoid}}(C_NULL)
     check(ctx.h, ccall((:b2k_op_create_csc, lib), Cint,
@@ -206,6 +208,20 @@ function apply_adjoint(A::B200Dense, x::B200Vec)                                
     return y
 end
 apply(A::B200Dense, x::B200Vec) = apply_normal(A, x)
+# A' of a CSR operator, assembled on the device from A's arrays (b2k_op_create_transpose): the CSR of A' with sorted
+# columns, so products with it have the bits of a host-built transpose.  apply_adjoint builds it once per operator,
+# which lets KrylovKit's own bieigsolve, svdsolve and lssolve take a B200CSR.
+function Base.adjoint(A::B200CSR{T}) where {T}
+    h = Ref{Ptr{Cvoid}}(C_NULL)
+    check(A.ctx.h, ccall((:b2k_op_create_transpose, lib), Cint, (Ptr{Cvoid}, Ref{Ptr{Cvoid}}, Ptr{Cvoid}),
+                         A.ctx.h, h, A.h))
+    return B200CSR{T}(A.ctx, h[])
+end
+apply_normal(A::B200CSR, x::B200Vec) = apply(A, x)                               # apply.jl:14
+function apply_adjoint(A::B200CSR, x::B200Vec)                                   # apply.jl:15
+    A.adj === nothing && (A.adj = adjoint(A))
+    return apply(A.adj, x)
+end
 # (A x, A'(A x)) from ONE pass over the dense A — the building block of the flagged one-pass GKL step (no KrylovKit
 # counterpart: gkl.jl:308-323 calls apply_adjoint and apply_normal separately).  A gklrecurrence specialisation on
 # `GKLIterator{<:B200Dense}` would keep G = A'U next to U and recover A'u_{k+1} = (z - G c) / beta with unproject!!,

@@ -182,6 +182,13 @@ int32_t b2k_op_create_dense_splitmix(b2k_ctx* ctx, b2k_op** out, int64_t m_local
 int32_t b2k_op_destroy(b2k_ctx* ctx, b2k_op* op);
 int32_t b2k_op_info(const b2k_op* op, int64_t* n_rows, int64_t* n_cols, int64_t* nnz,
                     int32_t* kind);
+/* *out = a new CSR operator holding A' (n_cols x n_rows), built on the device from op's arrays (the matrix never
+ * goes through the host).  Row c of A' lists its columns in ascending order (a stable sort by column of CSR(A)), so
+ * the arrays are those b2k_op_create_csr builds from scipy's sorted A.T.tocsr(), and SpMV with the result gives the
+ * same bits.  Any shape; n_cols must be the length of a vector space of the context.  Assembled stencils included:
+ * the transpose of stencil(c) is stencil(c) with west/east, south/north and down/up swapped.  Matrix-free stencils,
+ * dense operators (use b2k_op_apply_adjoint) and row-sharded contexts: B2K_ENOTSUP.  Destroy with b2k_op_destroy. */
+int32_t b2k_op_create_transpose(b2k_ctx* ctx, b2k_op** out, const b2k_op* op);
 /* Copy the device CSR back (test support): arrays sized n_rows+1 / nnz / nnz. */
 int32_t b2k_op_csr_download(b2k_ctx* ctx, const b2k_op* op, int32_t* rowptr,
                             int32_t* colidx, void* vals);
@@ -249,6 +256,17 @@ int32_t b2k_bicgstab_chain(b2k_ctx* ctx, const b2k_op* op, b2k_vec x, b2k_vec r,
  * — src/orthonormal.jl:88-118.  h is a HOST vector (orthonormal.jl:374, arnoldi.jl:212). */
 int32_t b2k_basis_project(b2k_ctx* ctx, const b2k_vec* cols, int32_t k, b2k_vec x,
                           double alpha, double beta, double* h_host);
+/* G[i,j] = <X[i], Y[j]> for i < p, j < q, except the leading p0 x q0 block, which is not written (64 x 64 column
+ * blocks wholly inside it are not swept).  G_host column-major, leading dimension ldg >= p.  1 <= p, q <= 256,
+ * 0 <= p0 <= p, 0 <= q0 <= q.
+ * The cross Gram matrix of two bases (the oblique projection W'V of BiArnoldi, src/factorizations/biarnoldi.jl)
+ * in ONE sweep over the rows of both lists for p, q <= 64; larger lists are swept in 64 x 64 column blocks
+ * (each block reads its own X and Y columns).  Handles may be in any order, in any spaces of one length, and may
+ * repeat between X and Y.  Deterministic: per-thread fma chains in the vector type, then threads and CTAs summed
+ * in double in a fixed order (basis.cu).  One host synchronisation.  Bad sizes / null pointers: B2K_EINVAL;
+ * columns of different lengths: B2K_EDIM; row-sharded contexts: B2K_ENOTSUP.  A refused call writes nothing. */
+int32_t b2k_basis_cross_inner(b2k_ctx* ctx, const b2k_vec* X, int32_t p, const b2k_vec* Y, int32_t q,
+                              int32_t p0, int32_t q0, double* G_host, int32_t ldg);
 /* unproject!!(y, b, c, alpha, beta, r): y = beta*y + alpha*sum_j b[cols[j]]*c[j]
  * — src/orthonormal.jl:132-196; also Base.:*(b, x) orthonormal.jl:57-60, the GMRES
  * x-update gmres.jl:105-108 and Ritz vectors eigsolve/lanczos.jl:131-133.

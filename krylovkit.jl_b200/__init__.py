@@ -10,14 +10,14 @@ B200Context does, and fails loudly without one (no CPU fallback).
 """
 from . import _lib
 from ._lib import B200Error, DimensionMismatch, LibraryMissing
-from .algorithms import (Arnoldi, BiCGStab, BlockLanczos, CG, ClassicalGramSchmidt, ClassicalGramSchmidt2,
+from .algorithms import (Arnoldi, BiArnoldi, BiCGStab, BlockLanczos, CG, ClassicalGramSchmidt, ClassicalGramSchmidt2,
                          ClassicalGramSchmidtIR, ConvergenceInfo, GKL, GMRES, KrylovDefaults,
                          Lanczos, LSMR, ModifiedGramSchmidt, ModifiedGramSchmidt2,
                          ModifiedGramSchmidt2Blocked, ModifiedGramSchmidtIR, Orthogonalizer, cgs, cgs2, cgsr, mgs,
                          mgs2, mgs2b, mgsr)
 from .operators import (B200CSR, B200Dense, B200Operator, apply, apply_adjoint, apply_normal,
                         apply_normal_gram)
-from .orthonormal import (OrthonormalBasis, basistransform_, orthogonalize_, orthonormalize_,
+from .orthonormal import (OrthonormalBasis, basistransform_, cross_inner, orthogonalize_, orthonormalize_,
                           project_, rank1update_, rmul_givens_, rmul_householder_, unproject_)
 from .vectors import B200Context, B200Vec, cache_release, inner, norm
 
@@ -29,6 +29,7 @@ from .schursolve import ComplexVec, realeigsolve, schursolve
 from .lssolve import lssolve
 from .expintegrator import expintegrator, exponentiate
 from .svdsolve import svdsolve
+from .bieigsolve import bieigsolve
 from . import factorizations
 from .factorizations.blocklanczos import Block
 

@@ -89,6 +89,7 @@ _PROTOS = {
     "b2k_op_destroy": (C.c_int32, [c_ctx, c_op]),
     "b2k_op_info": (C.c_int32, [c_op, P(C.c_int64), P(C.c_int64), P(C.c_int64), P(C.c_int32)]),
     "b2k_op_csr_download": (C.c_int32, [c_ctx, c_op, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "b2k_op_create_transpose": (C.c_int32, [c_ctx, P(c_op), c_op]),
     "b2k_op_apply": (C.c_int32, [c_ctx, c_op, c_vec, c_vec]),
     "b2k_op_apply_shifted": (C.c_int32, [c_ctx, c_op, c_vec, c_vec, C.c_double, C.c_double]),
     "b2k_op_apply_adjoint": (C.c_int32, [c_ctx, c_op, c_vec, c_vec]),
@@ -107,6 +108,8 @@ _PROTOS = {
                            [C.c_int32, P(C.c_double), P(C.c_int32)]),
     "b2k_basis_project": (C.c_int32, [c_ctx, P(c_vec), C.c_int32, c_vec, C.c_double, C.c_double,
                                       P(C.c_double)]),
+    "b2k_basis_cross_inner": (C.c_int32, [c_ctx, P(c_vec), C.c_int32, P(c_vec), C.c_int32, C.c_int32, C.c_int32,
+                                          P(C.c_double), C.c_int32]),
     "b2k_basis_unproject": (C.c_int32, [c_ctx, c_vec, P(c_vec), C.c_int32, P(C.c_double), C.c_double,
                                         C.c_double]),
     "b2k_basis_orthogonalize": (C.c_int32, [c_ctx, c_vec, P(c_vec), C.c_int32, P(C.c_double),

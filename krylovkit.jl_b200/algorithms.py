@@ -123,6 +123,17 @@ class Arnoldi:
 
 
 @dataclass(frozen=True)
+class BiArnoldi:
+    """src/algorithms.jl:255-291: the two-sided Krylov-Schur method of bieigsolve."""
+    orth: Orthogonalizer = field(default_factory=lambda: KrylovDefaults.orth)
+    krylovdim: int = KrylovDefaults.krylovdim
+    maxiter: int = KrylovDefaults.maxiter
+    tol: float = KrylovDefaults.tol
+    eager: bool = False
+    verbosity: int = KrylovDefaults.verbosity
+
+
+@dataclass(frozen=True)
 class GKL:
     orth: Orthogonalizer = field(default_factory=lambda: KrylovDefaults.orth)
     krylovdim: int = KrylovDefaults.krylovdim

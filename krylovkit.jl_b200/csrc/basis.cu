@@ -1348,6 +1348,8 @@ int32_t mgs_sweep(b2k_ctx* ctx, const Panel& pn, const VecRef& v, int k, int res
 
 }  // namespace
 
+int32_t b2k_cross_init(b2k_ctx* ctx);     // b2k_basis_cross_inner, below
+
 // called once per context (ctx.cu): opt in to > 48 KB dynamic shared memory
 int32_t b2k_basis_init(b2k_ctx* ctx) {
     if (const char* e = getenv("B2K_L2_HINTS")) g_l2_hints = e[0] != '0';
@@ -1379,7 +1381,7 @@ int32_t b2k_basis_init(b2k_ctx* ctx) {
     SETATTR(k_transform_big<double>, TB_SMEM_MAX);
     SETATTR(k_transform_big<float>, TB_SMEM_MAX);
 #undef SETATTR
-    return B2K_OK;
+    return b2k_cross_init(ctx);
 }
 
 extern "C" int32_t b2k_debug_set_dmma(int32_t on) {
@@ -2282,4 +2284,273 @@ extern "C" int32_t b2k_debug_trace_read(b2k_ctx* ctx, unsigned long long* out, i
     B2K_CUDA(ctx, cudaMemcpy(out, ctx->d_trace + 2, sizeof(unsigned long long) * 2 * cnt, cudaMemcpyDeviceToHost));
     *n_events = (int64_t)cnt;
     return B2K_OK;
+}
+
+// ------------------------------------------------------------------ cross Gram ----
+// b2k_basis_cross_inner: G[i, j] = <X[i], Y[j]> for two lists of columns, in ONE sweep over the rows per column block.
+//
+// A column block is at most CI_B = 64 columns of X times at most CI_B columns of Y (the single-pass limit: 256 threads
+// x a 4 x 4 register tile = 64 x 64 accumulators; it does not depend on the dtype).  Larger lists are split into
+// ceil(p/64) x ceil(q/64) blocks and each block is one sweep that reads its own X and Y columns, so a split call
+// reads  sum over blocks of (pb + qb) n sizeof(T)  bytes = (ceil(q/64) p + ceil(p/64) q) n sizeof(T)  instead of
+// (p + q) n sizeof(T).  Blocks that lie wholly inside the skip block are not swept.
+//
+// Kernel: one CTA per SM (grid = min(ceil(n / 64), #SMs)), CTA g owns row tiles g, g + grid, ... of CI_R = 64 rows.
+// A producer warp streams each tile's pb + qb column segments into a ring of shared-memory stages with 1-D TMA bulk
+// copies (one per column, completion on the stage's mbarrier, as in tsk.cuh); 8 consumer warps form the tile's
+// X_tile' Y_tile contribution in registers.  Consumer thread t = s * NO + o owns the 16 entries of entry tile
+// o = (oi, oj) — rows oi + a OI, columns oj + b OJ of the block, a, b < 4, OI = ceil(pb/4), OJ = ceil(qb/4),
+// NO = OI OJ — and row slice s < RS, where RS is the largest power of two <= min(32, 256 / NO): it reads the rows
+// r of the tile with r % RS == s.  Shared memory: nst (pb + qb) (64 + pad) sizeof(T) for the ring
+// (pad = 16 bytes, which spreads the columns of one row over the banks), plus 16 RS NO doubles for the slice sums.
+//
+// Rounding contract (the PROJECT phase of tsk.cuh): a thread accumulates its rows in the vector type T with an fma
+// chain, a = fma(X[r, i], Y[r, j], a) from a = 0, over its tiles in ascending order and its rows of each tile in
+// ascending order; the RS slice values of an entry are converted to double and added in slice order (from 0.0), and
+// the per-CTA values are added in CTA order (from 0.0) by k_cross_finalize.  No FP atomics: the bits depend only on
+// n, p, q, the column block and the number of SMs.  Launches per call: 2 per column block that is swept (the sweep
+// and k_cross_finalize); none when n == 0 or everything is skipped.  One host synchronisation per call.
+namespace {
+
+constexpr int CI_B = 64;                 // columns of X / of Y per block (the single-pass limit)
+constexpr int CI_R = 64;                 // rows per tile
+constexpr int CI_THREADS = 256 + 32;     // 8 consumer warps + 1 producer warp
+constexpr int CI_PART = CI_B * CI_B;     // doubles per CTA partial block
+constexpr int CI_SMEM_MAX = 232448;
+constexpr int CI_MAXLIST = 256;
+
+template <typename T> constexpr int ci_pitch() { return CI_R + 16 / (int)sizeof(T); }
+
+template <typename T>
+struct CrossParams {
+    const T* x[CI_B];
+    const T* y[CI_B];
+    int64_t n;
+    int pb, qb;          // block shape
+    int oj, no, rs;      // owner tiles per row of tiles, owner tiles, row slices
+    int skip_i, skip_j;  // entries (i < skip_i, j < skip_j) of the block are not wanted
+    int nst;             // ring stages
+    double* part;        // [grid][CI_PART]
+};
+
+template <typename T>
+__global__ void __launch_bounds__(CI_THREADS, 1) k_cross_inner(const __grid_constant__ CrossParams<T> p) {
+    extern __shared__ __align__(128) uint8_t ci_smem[];
+    constexpr int P = ci_pitch<T>();
+    const int ncol = p.pb + p.qb;
+    const uint32_t stage_bytes = (uint32_t)(ncol * P * sizeof(T));
+    double* red = reinterpret_cast<double*>(ci_smem + (size_t)p.nst * stage_bytes);
+    uint64_t* bars = reinterpret_cast<uint64_t*>(red + 16 * p.rs * p.no);
+    const uint32_t full = smem_u32(bars), empty = full + 8 * p.nst;
+    const uint32_t ring = smem_u32(ci_smem);
+    const int tid = threadIdx.x;
+    const int64_t ntiles = (p.n + CI_R - 1) / CI_R;
+    if (tid == 0) {
+        for (int i = 0; i < p.nst; ++i) {
+            mbar_init(full + 8 * i, 1);
+            mbar_init(empty + 8 * i, 8);
+        }
+        fence_mbar_init();
+    }
+    __syncthreads();
+
+    if (tid >= 256) {     // producer warp
+        const int lane = tid & 31;
+        int it = 0;
+        for (int64_t tile = blockIdx.x; tile < ntiles; tile += gridDim.x, ++it) {
+            const int s = it % p.nst;
+            const uint32_t ph = (uint32_t)((it / p.nst) & 1);
+            mbar_wait(empty + 8 * s, ph ^ 1);
+            const int64_t r0 = tile * CI_R;
+            const int rt = (int)((p.n - r0) < CI_R ? (p.n - r0) : CI_R);
+            const uint32_t bytes = (uint32_t)((rt * sizeof(T) + 15) & ~(size_t)15);
+            if (lane == 0) mbar_expect_tx(full + 8 * s, bytes * (uint32_t)ncol);
+            __syncwarp();
+            for (int c = lane; c < ncol; c += 32) {
+                const T* src = (c < p.pb ? p.x[c] : p.y[c - p.pb]) + r0;
+                bulk_g2s(ring + s * stage_bytes + c * P * (uint32_t)sizeof(T), src, bytes, full + 8 * s);
+            }
+        }
+        return;
+    }
+
+    // consumers
+    const int lane = tid & 31;
+    const int sl = tid / p.no, o = tid % p.no;
+    const bool active = sl < p.rs;
+    // entry tile o = (oi, oj) holds the entries (oi + a OI, oj + b OJ): the lanes of a warp read neighbouring
+    // columns, whose segments the 16-byte pad spreads over the banks
+    const int OI = p.no / p.oj;
+    const int oi = o / p.oj, oj = o % p.oj;
+    // a tile wholly inside the skip block does no arithmetic
+    const bool work = active && !(oi + 3 * OI < p.skip_i && oj + 3 * p.oj < p.skip_j);
+    int xi[4], yj[4];
+#pragma unroll
+    for (int a = 0; a < 4; ++a) {
+        xi[a] = min(oi + a * OI, p.pb - 1) * P;                // clamped: entries past the block are discarded
+        yj[a] = (p.pb + min(oj + a * p.oj, p.qb - 1)) * P;
+    }
+    T acc[4][4];
+#pragma unroll
+    for (int a = 0; a < 4; ++a)
+#pragma unroll
+        for (int b = 0; b < 4; ++b) acc[a][b] = (T)0;
+    int it = 0;
+    for (int64_t tile = blockIdx.x; tile < ntiles; tile += gridDim.x, ++it) {
+        const int s = it % p.nst;
+        const uint32_t ph = (uint32_t)((it / p.nst) & 1);
+        mbar_wait(full + 8 * s, ph);
+        const int64_t r0 = tile * CI_R;
+        const int rt = (int)((p.n - r0) < CI_R ? (p.n - r0) : CI_R);
+        const T* st = reinterpret_cast<const T*>(ci_smem + (size_t)s * stage_bytes);
+        if (work) {
+            for (int r = sl; r < rt; r += p.rs) {
+                T xv[4], yv[4];
+#pragma unroll
+                for (int a = 0; a < 4; ++a) { xv[a] = st[xi[a] + r]; yv[a] = st[yj[a] + r]; }
+#pragma unroll
+                for (int a = 0; a < 4; ++a)
+#pragma unroll
+                    for (int b = 0; b < 4; ++b) acc[a][b] = fma(xv[a], yv[b], acc[a][b]);
+            }
+        }
+        __syncwarp();
+        if (lane == 0) mbar_arrive(empty + 8 * s);
+    }
+
+    // slice sums in slice order, in double
+    if (active) {
+        double* mine = red + (size_t)(sl * p.no + o) * 16;
+#pragma unroll
+        for (int a = 0; a < 4; ++a)
+#pragma unroll
+            for (int b = 0; b < 4; ++b) mine[a * 4 + b] = (double)acc[a][b];
+    }
+    named_bar_sync(1, 256);
+    double* part = p.part + (size_t)blockIdx.x * CI_PART;
+    for (int e = tid; e < p.pb * p.qb; e += 256) {
+        const int i = e % p.pb, j = e / p.pb;
+        const int OI = p.no / p.oj;
+        const int oo = (i % OI) * p.oj + j % p.oj, ab = (i / OI) * 4 + j / p.oj;
+        double v = 0.0;
+        for (int s2 = 0; s2 < p.rs; ++s2) v += red[(size_t)(s2 * p.no + oo) * 16 + ab];
+        part[e] = v;
+    }
+}
+
+// G[(j0 + j) * ldg + i0 + i] = sum over CTAs g in order of part[g][i + j pb], outside the skip block
+__global__ void __launch_bounds__(256) k_cross_finalize(const double* __restrict__ part, int grid, int pb, int qb,
+                                                        int i0, int j0, int p0, int q0, double* __restrict__ G,
+                                                        int ldg) {
+    const int e = blockIdx.x * 256 + threadIdx.x;
+    if (e >= pb * qb) return;
+    const int i = e % pb, j = e / pb;
+    if (i0 + i < p0 && j0 + j < q0) return;
+    double v = 0.0;
+    for (int g = 0; g < grid; ++g) v += part[(size_t)g * CI_PART + e];
+    G[(size_t)(j0 + j) * ldg + i0 + i] = v;
+}
+
+template <typename T>
+int32_t cross_block(b2k_ctx* ctx, const std::vector<VecRef>& X, const std::vector<VecRef>& Y, int i0, int pb,
+                    int j0, int qb, int p0, int q0, int64_t n, double* d_part, double* d_G, int ldg) {
+    CrossParams<T> cp;
+    memset(&cp, 0, sizeof(cp));
+    for (int i = 0; i < pb; ++i) cp.x[i] = (const T*)X[i0 + i].ptr;
+    for (int j = 0; j < qb; ++j) cp.y[j] = (const T*)Y[j0 + j].ptr;
+    cp.n = n;
+    cp.pb = pb;
+    cp.qb = qb;
+    cp.oj = (qb + 3) / 4;
+    cp.no = ((pb + 3) / 4) * cp.oj;
+    cp.rs = 1;
+    while (cp.rs * 2 <= 32 && cp.rs * 2 * cp.no <= 256) cp.rs *= 2;
+    cp.skip_i = std::max(0, std::min(p0 - i0, pb));
+    cp.skip_j = std::max(0, std::min(q0 - j0, qb));
+    const size_t stage = (size_t)(pb + qb) * ci_pitch<T>() * sizeof(T);
+    const size_t red = (size_t)16 * cp.rs * cp.no * sizeof(double);
+    cp.nst = (int)std::max<size_t>(2, std::min<size_t>(6, (200 * 1024 - red) / stage));
+    const size_t smem = cp.nst * stage + red + 16 * (size_t)cp.nst;
+    if (smem > (size_t)CI_SMEM_MAX) return b2k_fail(ctx, B2K_ENOTSUP, "basis_cross_inner: shared memory");
+    const int64_t ntiles = (n + CI_R - 1) / CI_R;
+    const int grid = (int)std::min<int64_t>(ntiles, ctx->num_sms);
+    cp.part = d_part;
+    const int pr = b2k_prof_begin(ctx, 9, (double)(pb + qb) * sizeof(T) * (double)n);
+    k_cross_inner<T><<<grid, CI_THREADS, smem, ctx->stream>>>(cp);
+    B2K_LAUNCH_CHECK(ctx);
+    b2k_prof_end(ctx, pr);
+    k_cross_finalize<<<(pb * qb + 255) / 256, 256, 0, ctx->stream>>>(d_part, grid, pb, qb, i0, j0, p0, q0, d_G, ldg);
+    B2K_LAUNCH_CHECK(ctx);
+    return B2K_OK;
+}
+
+}  // namespace
+
+int32_t b2k_cross_init(b2k_ctx* ctx) {
+    B2K_CUDA(ctx, cudaFuncSetAttribute(k_cross_inner<double>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                       CI_SMEM_MAX));
+    B2K_CUDA(ctx, cudaFuncSetAttribute(k_cross_inner<float>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                       CI_SMEM_MAX));
+    return B2K_OK;
+}
+
+extern "C" int32_t b2k_basis_cross_inner(b2k_ctx* ctx, const b2k_vec* X, int32_t p, const b2k_vec* Y, int32_t q,
+                                         int32_t p0, int32_t q0, double* G_host, int32_t ldg) {
+    if (!ctx || !X || !Y || !G_host) return B2K_EINVAL;
+    if (p < 1 || q < 1 || p > CI_MAXLIST || q > CI_MAXLIST || p0 < 0 || p0 > p || q0 < 0 || q0 > q || ldg < p)
+        return b2k_fail(ctx, B2K_EINVAL, "basis_cross_inner: need 1 <= p, q <= %d, 0 <= p0 <= p, 0 <= q0 <= q, "
+                                         "ldg >= p (p = %d, q = %d, p0 = %d, q0 = %d, ldg = %d)",
+                        CI_MAXLIST, p, q, p0, q0, ldg);
+    if (ctx->nranks > 1)
+        return b2k_fail(ctx, B2K_ENOTSUP, "basis_cross_inner: row-sharded contexts are not supported");
+    std::vector<VecRef> xr(p), yr(q);
+    for (int i = 0; i < p; ++i) B2K_TRY(b2k_resolve(ctx, X[i], &xr[i]));
+    for (int j = 0; j < q; ++j) B2K_TRY(b2k_resolve(ctx, Y[j], &yr[j]));
+    const int64_t n = xr[0].n;
+    for (const VecRef& v : xr)
+        if (v.n != n) return b2k_fail(ctx, B2K_EDIM, "basis_cross_inner: columns of %lld and %lld rows",
+                                      (long long)n, (long long)v.n);
+    for (const VecRef& v : yr)
+        if (v.n != n) return b2k_fail(ctx, B2K_EDIM, "basis_cross_inner: columns of %lld and %lld rows",
+                                      (long long)n, (long long)v.n);
+    if (p0 == p && q0 == q) return B2K_OK;
+    if (n == 0) {
+        for (int j = 0; j < q; ++j)
+            for (int i = 0; i < p; ++i)
+                if (!(i < p0 && j < q0)) G_host[(size_t)j * ldg + i] = 0.0;
+        return B2K_OK;
+    }
+    B2K_CUDA(ctx, cudaSetDevice(ctx->device));
+    const int grid = (int)std::min<int64_t>((n + CI_R - 1) / CI_R, ctx->num_sms);
+    double *d_part = nullptr, *d_G = nullptr, *h_G = nullptr;
+    const size_t gbytes = sizeof(double) * CI_MAXLIST * CI_MAXLIST;
+    auto release = [&]() {
+        if (d_part) B2K_DFREE(d_part);
+        if (d_G) B2K_DFREE(d_G);
+        if (h_G) b2k_hfree(h_G, gbytes);
+    };
+    int32_t rc = B2K_OK;
+    if (B2K_DMALLOC(&d_part, sizeof(double) * (size_t)grid * CI_PART) != cudaSuccess ||
+        B2K_DMALLOC(&d_G, sizeof(double) * (size_t)p * q) != cudaSuccess || b2k_hmalloc((void**)&h_G, gbytes) != cudaSuccess)
+        rc = b2k_fail(ctx, B2K_ENOMEM, "basis_cross_inner: staging allocation failed");
+    for (int i0 = 0; rc == B2K_OK && i0 < p; i0 += CI_B)
+        for (int j0 = 0; rc == B2K_OK && j0 < q; j0 += CI_B) {
+            const int pb = std::min(CI_B, p - i0), qb = std::min(CI_B, q - j0);
+            if (i0 + pb <= p0 && j0 + qb <= q0) continue;
+            rc = ctx->dtype == B2K_F64
+                     ? cross_block<double>(ctx, xr, yr, i0, pb, j0, qb, p0, q0, n, d_part, d_G, p)
+                     : cross_block<float>(ctx, xr, yr, i0, pb, j0, qb, p0, q0, n, d_part, d_G, p);
+        }
+    if (rc == B2K_OK) {
+        const cudaError_t e = cudaMemcpyAsync(h_G, d_G, sizeof(double) * (size_t)p * q, cudaMemcpyDeviceToHost,
+                                              ctx->stream);
+        if (e != cudaSuccess) rc = b2k_fail(ctx, B2K_ECUDA, "basis_cross_inner: %s", cudaGetErrorString(e));
+    }
+    if (rc == B2K_OK) rc = b2k_stream_sync(ctx);
+    if (rc == B2K_OK)
+        for (int j = 0; j < q; ++j)
+            for (int i = 0; i < p; ++i)
+                if (!(i < p0 && j < q0)) G_host[(size_t)j * ldg + i] = h_G[(size_t)j * p + i];
+    release();
+    return rc;
 }

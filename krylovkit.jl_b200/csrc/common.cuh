@@ -38,8 +38,8 @@ struct B2kNccl;   // dist.cu
 
 // optional per-kernel-class timing (CUDA events on the context stream), used by bench.py
 // for the roofline figure: class 0 = CSR SpMV, 1 = fused Gram-Schmidt, 2 = basis transform,
-// 3 = project, 4 = unproject
-constexpr int B2K_PROF_CLASSES = 9;
+// 3 = project, 4 = unproject, ..., 9 = cross Gram sweep (b2k_basis_cross_inner)
+constexpr int B2K_PROF_CLASSES = 10;
 struct B2kProfRec { int cls; double bytes; cudaEvent_t e0, e1; };
 struct B2kProf {
     bool on = false;

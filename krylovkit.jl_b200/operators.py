@@ -127,6 +127,17 @@ class B200CSR(B200Operator):
         ctx.check(ctx.lib.b2k_op_create_stencil_free(ctx.h, C.byref(h), nx, ny, nz, c))
         return cls(ctx, h)
 
+    def transpose(self) -> "B200CSR":
+        """A' as a new device CSR operator, built on the device (b2k_op_create_transpose): the arrays of scipy's
+        sorted A.T.tocsr(), so products with it are bit-identical to those with the host-built transpose.  Spaces
+        given explicitly to A are swapped.  Not for matrix-free stencils or row-sharded contexts."""
+        h = L.c_op()
+        self.ctx.check(self.ctx.lib.b2k_op_create_transpose(self.ctx.h, C.byref(h), self.h))
+        t = B200CSR(self.ctx, h)
+        if self._explicit_spaces:
+            t.with_spaces(self.space_out, self.space_in)
+        return t
+
     def to_scipy(self):
         import scipy.sparse as sp
         rp = np.empty(self.n_rows + 1, dtype=np.int32)

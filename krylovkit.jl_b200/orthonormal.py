@@ -70,6 +70,25 @@ def _cols(b: OrthonormalBasis, r):
     return vecs, handles(vecs)
 
 
+def cross_inner(X, Y, skip=(0, 0), G: np.ndarray | None = None) -> np.ndarray:
+    """G[i, j] = <X[i], Y[j]> (host float64, column-major p x q) in one device sweep over both lists —
+    b2k_basis_cross_inner.  X and Y are sequences of B200Vec (or OrthonormalBasis), at most 256 each.  The leading
+    skip = (p0, q0) block of G is neither computed nor written: pass the G of an earlier call to update only the
+    rows and columns added since then."""
+    X, Y = list(X), list(Y)
+    p, q = len(X), len(Y)
+    if G is None:
+        G = np.zeros((p, q), order="F")
+    if G.dtype != np.float64 or not G.flags.f_contiguous or G.shape[0] < p or G.shape[1] < q:
+        raise ValueError("cross_inner: G must be a Fortran-ordered float64 array of at least p x q")
+    if p == 0 or q == 0:
+        return G
+    ctx = X[0].ctx
+    ctx.check(ctx.lib.b2k_basis_cross_inner(ctx.h, handles(X), p, handles(Y), q, int(skip[0]), int(skip[1]),
+                                            G.ctypes.data_as(C.POINTER(C.c_double)), G.shape[0]))
+    return G
+
+
 def project_(y: np.ndarray, b: OrthonormalBasis, x: B200Vec, alpha: float = 1.0, beta: float = 0.0,
              r=None) -> np.ndarray:
     """project!!(y, b, x, α, β, r): y[j] = β y[j] + α <b[r[j]], x> — orthonormal.jl:88-118.
