@@ -20,7 +20,7 @@ import KrylovKit: LanczosIterator, LanczosFactorization, expand!, normres
 import KrylovKit: ClassicalGramSchmidt, ModifiedGramSchmidt, ClassicalGramSchmidt2, ModifiedGramSchmidt2,
     ClassicalGramSchmidtIR, ModifiedGramSchmidtIR
 
-export B200Ctx, B200Vec, B200CSR, B200Dense
+export B200Ctx, B200Vec, B200CSR, B200Dense, B200Pencil
 
 const lib = get(ENV, "B200KRYLOV_LIB", "libb200krylov.so")
 
@@ -222,6 +222,78 @@ function apply_adjoint(A::B200CSR, x::B200Vec)                                  
     A.adj === nothing && (A.adj = adjoint(A))
     return apply(A.adj, x)
 end
+# The pencil (A, B) of geneigsolve (b2k_pencil_*): one fused pass over both matrices per product when their CSR
+# patterns are equal, separate products otherwise, the same bits either way.  Calling it gives (A x, B x), so
+# KrylovKit's `genapply(f, x) = f(x)` (apply.jl:23) takes it; golubyerecurrence is specialised below.
+mutable struct B200Pencil
+    ctx::B200Ctx
+    h::Ptr{Cvoid}
+    A::Any                                # keeps A and B alive as long as the pencil
+    B::Any
+end
+function B200Pencil(A::B200CSR, B::B200CSR)
+    h = Ref{Ptr{Cvoid}}(C_NULL)
+    check(A.ctx.h, ccall((:b2k_pencil_create, lib), Cint, (Ptr{Cvoid}, Ref{Ptr{Cvoid}}, Ptr{Cvoid}, Ptr{Cvoid}),
+                         A.ctx.h, h, A.h, B.h))
+    P = B200Pencil(A.ctx, h[], A, B)
+    finalizer(P) do p
+        p.ctx.h == C_NULL || ccall((:b2k_pencil_destroy, lib), Cint, (Ptr{Cvoid}, Ptr{Cvoid}), p.ctx.h, p.h)
+    end
+    return P
+end
+function (P::B200Pencil)(x::B200Vec)                                           # genapply, golubye.jl:9, 112
+    ax, bx = B200Vec(x.ctx; space = space(x)), B200Vec(x.ctx; space = space(x))
+    check(x.ctx.h, ccall((:b2k_pencil_rayleigh, lib), Cint,
+                         (Ptr{Cvoid}, Ptr{Cvoid}, Int32, Int32, Int32, Ptr{Float64}, Ptr{Float64}),
+                         x.ctx.h, P.h, x.handle, ax.handle, bx.handle, C_NULL, C_NULL))
+    return ax, bx
+end
+# golubyerecurrence (golubye.jl:196-284) with the product, the shift, the MGS-order `add!!(w, V[end-1], -β)` and the
+# first inner product from one b2k_pencil_apply; the rest of each variant is the reference's own code path.
+function KrylovKit.golubyerecurrence(P::B200Pencil, ρ, V::OrthonormalBasis, β, orth::Orthogonalizer)
+    v = V[end]
+    w, bv = B200Vec(v.ctx; space = space(v)), B200Vec(v.ctx; space = space(v))
+    mgs = orth isa Union{ModifiedGramSchmidt, ModifiedGramSchmidt2, ModifiedGramSchmidtIR}
+    s = Ref{Float64}(0.0)
+    check(v.ctx.h, ccall((:b2k_pencil_apply, lib), Cint,
+                         (Ptr{Cvoid}, Ptr{Cvoid}, Int32, Int32, Int32, Float64, Int32, Float64, Ref{Float64}),
+                         v.ctx.h, P.h, v.handle, w.handle, bv.handle, Float64(ρ), mgs ? V[end - 1].handle : Int32(-1),
+                         Float64(β), s))
+    α = s[]
+    mgs || (w = add!!(w, V[end - 1], -β))
+    w = add!!(w, v, -α)
+    if orth isa ClassicalGramSchmidt2
+        w, c = orthogonalize!!(w, V, ClassicalGramSchmidt())
+        α += c[end]
+    elseif orth isa ModifiedGramSchmidt2
+        c = α
+        for q in V
+            w, c = orthogonalize!!(w, q, ModifiedGramSchmidt())
+        end
+        α += c
+    elseif orth isa Union{ClassicalGramSchmidtIR, ModifiedGramSchmidtIR}
+        ab2 = abs2(α) + abs2(β)
+        β = norm(w)
+        nold = sqrt(abs2(β) + ab2)
+        while eps(one(β)) < β < orth.η * nold
+            nold = β
+            if orth isa ClassicalGramSchmidtIR
+                w, c = orthogonalize!!(w, V, ClassicalGramSchmidt())
+                α += c[end]
+            else
+                c = zero(α)
+                for q in V
+                    w, c = orthogonalize!!(w, q, ModifiedGramSchmidt())
+                end
+                α += c
+            end
+            β = norm(w)
+        end
+        return w, α, β, bv
+    end
+    return w, α, norm(w), bv
+end
+
 # (A x, A'(A x)) from ONE pass over the dense A — the building block of the flagged one-pass GKL step (no KrylovKit
 # counterpart: gkl.jl:308-323 calls apply_adjoint and apply_normal separately).  A gklrecurrence specialisation on
 # `GKLIterator{<:B200Dense}` would keep G = A'U next to U and recover A'u_{k+1} = (z - G c) / beta with unproject!!,

@@ -210,6 +210,30 @@ int32_t b2k_op_apply_normal_gram(b2k_ctx* ctx, const b2k_op* op, b2k_vec x, b2k_
 int32_t b2k_op_apply_dot(b2k_ctx* ctx, const b2k_op* op, b2k_vec x, b2k_vec y, b2k_vec v,
                          double* dot);
 
+/* Pencil (A, B) of geneigsolve / Golub-Ye (src/eigsolve/golubye.jl): two square operators of one context, of one
+ * size.  Keeps references to A and B (destroy the pencil first).  Compares the CSR patterns ON THE DEVICE once
+ * (rowptr and colidx equal) to pick the fused path, one pass over both matrices per call; any other pair
+ * (different patterns, matrix-free stencil, dense) takes the composed path of b2k_op_apply / b2k_vec_axpby /
+ * b2k_vec_inner.  Row-sharded contexts: B2K_ENOTSUP.  Different sizes / non-square: B2K_EDIM.  A == B or an
+ * operator of another context: B2K_EINVAL.  The handle is opaque (struct b2k_pencil) and travels as a void*. */
+int32_t b2k_pencil_create(b2k_ctx* ctx, void** out, const b2k_op* A, const b2k_op* B);
+int32_t b2k_pencil_destroy(b2k_ctx* ctx, void* P);
+/* golubyerecurrence's product, golubye.jl:198-199 (+202/211 when vprev >= 0):
+ *   bx = B x;  w = add!!(A x, bx, -rho)  i.e. w[r] = fma(-rho, bx[r], (A x)[r]);
+ *   if vprev >= 0:  w[r] = fma(-beta, vprev[r], w[r])          (add!!(w, V[end-1], -β), MGS order)
+ *   if dot != NULL: *dot = <x, w>  (of the final w)
+ * w and bx are bit-identical on both paths to b2k_op_apply with A and B followed by b2k_vec_axpby(w, bx, -rho, 1) and
+ * b2k_vec_axpby(w, vprev, -beta, 1).  The dot of the fused path is a deterministic per-CTA sum (as b2k_op_apply_dot)
+ * and may differ from b2k_vec_inner in the last bits.  w, bx, x, vprev pairwise distinct; a refused call writes
+ * nothing. */
+int32_t b2k_pencil_apply(b2k_ctx* ctx, const void* P, b2k_vec x, b2k_vec w, b2k_vec bx, double rho,
+                         b2k_vec vprev, double beta, double* dot);
+/* genapply and both Rayleigh inner products in one pass (golubye.jl:9-14, 112-114): ax = A x, bx = B x,
+ * *xax = <x, ax>, *xbx = <x, bx> (each pointer may be NULL: that dot is not returned).  Same rounding contract as
+ * b2k_pencil_apply; x, ax, bx pairwise distinct. */
+int32_t b2k_pencil_rayleigh(b2k_ctx* ctx, const void* P, b2k_vec x, b2k_vec ax, b2k_vec bx,
+                            double* xax, double* xbx);
+
 /* One conjugate-gradient iteration (SURVEY §8f-2, src/linsolve/cg.jl:62-67) with one host round trip:
  * p <- beta*p + r; q <- (a0 + a1*A) p fused with <p,q>; alpha = rho/<p,q> (on the device);
  * x += alpha*p; r -= alpha*q; returns <p,q> and ||r||.  beta = 0 is the first iteration (p = r). */

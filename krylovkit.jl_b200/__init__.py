@@ -11,12 +11,12 @@ B200Context does, and fails loudly without one (no CPU fallback).
 from . import _lib
 from ._lib import B200Error, DimensionMismatch, LibraryMissing
 from .algorithms import (Arnoldi, BiArnoldi, BiCGStab, BlockLanczos, CG, ClassicalGramSchmidt, ClassicalGramSchmidt2,
-                         ClassicalGramSchmidtIR, ConvergenceInfo, GKL, GMRES, KrylovDefaults,
+                         ClassicalGramSchmidtIR, ConvergenceInfo, GKL, GMRES, GolubYe, KrylovDefaults,
                          Lanczos, LSMR, ModifiedGramSchmidt, ModifiedGramSchmidt2,
                          ModifiedGramSchmidt2Blocked, ModifiedGramSchmidtIR, Orthogonalizer, cgs, cgs2, cgsr, mgs,
                          mgs2, mgs2b, mgsr)
-from .operators import (B200CSR, B200Dense, B200Operator, apply, apply_adjoint, apply_normal,
-                        apply_normal_gram)
+from .operators import (B200CSR, B200Dense, B200Operator, B200Pencil, apply, apply_adjoint, apply_normal,
+                        apply_normal_gram, genapply)
 from .orthonormal import (OrthonormalBasis, basistransform_, cross_inner, orthogonalize_, orthonormalize_,
                           project_, rank1update_, rmul_givens_, rmul_householder_, unproject_)
 from .vectors import B200Context, B200Vec, cache_release, inner, norm
@@ -30,6 +30,7 @@ from .lssolve import lssolve
 from .expintegrator import expintegrator, exponentiate
 from .svdsolve import svdsolve
 from .bieigsolve import bieigsolve
+from .geneigsolve import geneigselector, geneigsolve
 from . import factorizations
 from .factorizations.blocklanczos import Block
 

@@ -95,6 +95,11 @@ _PROTOS = {
     "b2k_op_apply_adjoint": (C.c_int32, [c_ctx, c_op, c_vec, c_vec]),
     "b2k_op_apply_normal_gram": (C.c_int32, [c_ctx, c_op, c_vec, c_vec, c_vec]),
     "b2k_op_apply_dot": (C.c_int32, [c_ctx, c_op, c_vec, c_vec, c_vec, P(C.c_double)]),
+    "b2k_pencil_create": (C.c_int32, [c_ctx, P(C.c_void_p), c_op, c_op]),
+    "b2k_pencil_destroy": (C.c_int32, [c_ctx, C.c_void_p]),
+    "b2k_pencil_apply": (C.c_int32, [c_ctx, C.c_void_p, c_vec, c_vec, c_vec, C.c_double, c_vec, C.c_double,
+                                     P(C.c_double)]),
+    "b2k_pencil_rayleigh": (C.c_int32, [c_ctx, C.c_void_p, c_vec, c_vec, c_vec, P(C.c_double), P(C.c_double)]),
     "b2k_cg_step": (C.c_int32, [c_ctx, c_op, c_vec, c_vec, c_vec, c_vec, C.c_double, C.c_double, C.c_double,
                                 C.c_double, P(C.c_double), P(C.c_double)]),
     "b2k_cg_chain": (C.c_int32, [c_ctx, c_op, c_vec, c_vec, c_vec, c_vec, C.c_double, C.c_double, C.c_double,
@@ -148,6 +153,7 @@ _PROTOS = {
     "b2k_debug_set_dmma": (C.c_int32, [C.c_int32]),
     "b2k_debug_set_transform": (C.c_int32, [C.c_int32]),
     "b2k_debug_transform_kernel": (C.c_int32, []),
+    "b2k_debug_pencil_path": (C.c_int32, []),
     "b2k_debug_set_chain": (C.c_int32, [C.c_int32]),
     "b2k_debug_used_columns": (C.c_int32, [c_ctx, C.c_int32]),
     "b2k_debug_set_chain_mode": (C.c_int32, [C.c_int32]),

@@ -134,6 +134,17 @@ class BiArnoldi:
 
 
 @dataclass(frozen=True)
+class GolubYe:
+    """src/algorithms.jl:310-325: the Golub-Ye method of geneigsolve for A x = λ B x with A symmetric and B symmetric
+    positive definite.  The reference struct has no `eager` field (its docstring mentions one)."""
+    orth: Orthogonalizer = field(default_factory=lambda: KrylovDefaults.orth)
+    krylovdim: int = KrylovDefaults.krylovdim
+    maxiter: int = KrylovDefaults.maxiter
+    tol: float = KrylovDefaults.tol
+    verbosity: int = KrylovDefaults.verbosity
+
+
+@dataclass(frozen=True)
 class GKL:
     orth: Orthogonalizer = field(default_factory=lambda: KrylovDefaults.orth)
     krylovdim: int = KrylovDefaults.krylovdim

@@ -427,6 +427,259 @@ k_spmv_pipe(const int32_t* __restrict__ rowptr, const int32_t* __restrict__ coli
     }
 }
 
+// ---------------------------------------------------------------------------------------
+// Fused two-operator SpMV of a pencil (A, B) whose CSR patterns are equal (b2k_pencil_apply / b2k_pencil_rayleigh):
+// golubyerecurrence's product `av, bv = genapply(f, v); w = add!!(av, bv, -ρ)` (golubye.jl:198-199, plus
+// `add!!(w, V[end-1], -β)` of :202/:211) and the genapply of the Ritz loop (:112-114).  k_spmv_pipe's structure with
+// B's values staged next to A's in every ring stage: rowptr and colidx are streamed once, x[c] is gathered once per
+// nonzero for both products, and only the outputs are written — 2 (sizeof(T) + 2) nnz + 4 (n + 1) + 3 sizeof(T) n
+// bytes instead of 2 (sizeof(T) + 4) nnz + 8 (n + 1) + ... for the composition.
+//
+// Rounding contract: every row of A x and of B x is formed exactly as k_spmv_pipe forms it — products rounded in T and
+// summed in CSR order in T; a long row (> SP_NNZ nonzeros in its tile) as a double sum of rounded products, thread i
+// taking nonzeros i, i + 256, ..., then warp butterflies, then the 8 warps in order, rounded to T once.  Then
+//   MODE 0: bx = B x;  w = fma(-rho, bx, A x);  w = fma(-beta, vprev, w) when vprev is given;
+//   MODE 1: ax = A x;  bx = B x;
+// so ax, bx and w are bit-identical to b2k_op_apply with A and with B followed by b2k_vec_axpby(w, bx, -rho, 1) and
+// b2k_vec_axpby(w, vprev, -beta, 1).  The dots (<x, w>; <x, ax> and <x, bx>) are fma chains in T over each thread's
+// rows, summed per CTA in double (warp butterflies, then the warps in order); the last CTA to take a ticket adds the
+// CTA partials in CTA order (the scheme of b2k_op_apply_dot, no FP atomics).  They may differ from b2k_vec_inner in
+// the last bits.
+//
+// A stage holds both value arrays: 35008 B in Float64 (22656 B in Float32), so two stages are 70 KB (45 KB) per CTA.
+// Float64 runs 3 CTAs per SM (210 KB; four would need 280 KB of the 227 KB), Float32 4 CTAs per SM (181 KB), the
+// shape of the default single-operator variant.  -Xptxas -v: no spills for either.
+template <typename T, int NSTG> struct PenLayout {
+    static constexpr int VAL_BYTES = SPP_TV * (int)sizeof(T);
+    static constexpr int COL_BYTES = SPP_TV * 4;
+    static constexpr int RP_BYTES = (SPP_RMAX + 8) * 4;
+    static constexpr int OFF_COL = 2 * VAL_BYTES;
+    static constexpr int OFF_RP = 2 * VAL_BYTES + COL_BYTES;
+    static constexpr int STAGE = 2 * VAL_BYTES + COL_BYTES + RP_BYTES;
+    static constexpr int OFF_BAR = NSTG * STAGE;
+    static constexpr int OFF_RED = OFF_BAR + 2 * NSTG * 8 + 16;
+    static constexpr int SMEM = OFF_RED + 32 * 8 + 16;
+};
+constexpr int PEN_NSTG = 2;
+template <typename T> struct PenCtas { static constexpr int N = sizeof(T) == 8 ? 3 : 4; };
+
+template <typename T, int MODE>
+__device__ __forceinline__ void pencil_row(int r, T sa, T sb, T xr, T vp, T nrho, T nbeta, bool has_prev, T* y0,
+                                           T* y1, bool hints, uint64_t pol, T& d0, T& d1) {
+    if (MODE == 0) {
+        T wv = fma(nrho, sb, sa);                       // add!!(av, bv, -ρ): k_axpby MODE 1
+        if (has_prev) wv = fma(nbeta, vp, wv);          // add!!(w, V[end-1], -β)
+        sa = wv;
+    } else {
+        d1 = fma(xr, sb, d1);
+    }
+    d0 = fma(xr, sa, d0);
+    if (hints) {
+        st_hint(y0 + r, sa, pol);
+        st_hint(y1 + r, sb, pol);
+    } else {
+        y0[r] = sa;
+        y1[r] = sb;
+    }
+}
+
+template <typename T, int NSTG, int MINB, int MODE>
+__global__ void __launch_bounds__(SPP_THREADS, MINB)
+k_spmv_pencil(const int32_t* __restrict__ rowptr, const int32_t* __restrict__ colidx, const T* __restrict__ va,
+              const T* __restrict__ vb, const T* __restrict__ x, T* __restrict__ y0, T* __restrict__ y1,
+              const int32_t* __restrict__ rowblk, const int32_t* __restrict__ pblk, int nblk, T nrho,
+              const T* __restrict__ vprev, T nbeta, int want_dot, int l2_hints, double* __restrict__ part,
+              unsigned* __restrict__ ticket, double* __restrict__ out) {
+    using LY = PenLayout<T, NSTG>;
+    extern __shared__ __align__(128) uint8_t smem[];
+    const uint32_t full = smem_u32(smem + LY::OFF_BAR), empty = full + NSTG * 8;
+    double* red = reinterpret_cast<double*>(smem + LY::OFF_RED);
+    int* flag = reinterpret_cast<int*>(smem + LY::OFF_RED + 32 * 8);
+    if (threadIdx.x == 0) {
+        for (int i = 0; i < NSTG; ++i) {
+            mbar_init(full + 8 * i, 1);
+            mbar_init(empty + 8 * i, SPP_CONS / 32);
+        }
+        fence_mbar_init();
+    }
+    __syncthreads();
+    const int lane = threadIdx.x & 31;
+    uint32_t s = 0, ph = 0;
+    if (threadIdx.x >= SPP_CONS) {
+        // ------------------------------ producer warp (k_spmv_pipe's, plus B's values) ------------------------------
+        int tile = blockIdx.x;
+        int d = 0;
+        if (tile < nblk && lane < 4) d = (lane < 2) ? rowblk[tile + lane] : pblk[tile + lane - 2];
+        for (; tile < nblk; tile += gridDim.x) {
+            const int r0 = __shfl_sync(0xffffffffu, d, 0), r1 = __shfl_sync(0xffffffffu, d, 1);
+            const int p0 = __shfl_sync(0xffffffffu, d, 2), p1 = __shfl_sync(0xffffffffu, d, 3);
+            const int nt = tile + gridDim.x;
+            if (nt < nblk && lane < 4) d = (lane < 2) ? rowblk[nt + lane] : pblk[nt + lane - 2];
+            mbar_wait(empty + 8 * s, ph ^ 1);
+            const int nnzb = p1 - p0, nrows = r1 - r0;
+            if (nnzb <= SP_NNZ) {
+                const int p0a = p0 & ~3, cnt = ((p1 + 3) & ~3) - p0a;
+                const int r0a = r0 & ~3;
+                const int rcnt = (nrows <= SPP_RMAX) ? (((r1 + 1 + 3) & ~3) - r0a) : 0;
+                const uint32_t vbyt = (uint32_t)cnt * (uint32_t)sizeof(T), cb = (uint32_t)cnt * 4u,
+                               rb = (uint32_t)rcnt * 4u;
+                const uint32_t st = smem_u32(smem + s * LY::STAGE);
+                if (lane == 0) mbar_expect_tx(full + 8 * s, 2 * vbyt + cb + rb);
+                __syncwarp();
+                if (l2_hints) {
+                    const uint64_t pol = l2_policy_evict_first();
+                    if (lane == 0 && vbyt) bulk_g2s_hint(st, va + p0a, vbyt, full + 8 * s, pol);
+                    if (lane == 3 && vbyt) bulk_g2s_hint(st + LY::VAL_BYTES, vb + p0a, vbyt, full + 8 * s, pol);
+                    if (lane == 1 && cb) bulk_g2s_hint(st + LY::OFF_COL, colidx + p0a, cb, full + 8 * s, pol);
+                    if (lane == 2 && rb) bulk_g2s_hint(st + LY::OFF_RP, rowptr + r0a, rb, full + 8 * s, pol);
+                } else {
+                    if (lane == 0 && vbyt) bulk_g2s(st, va + p0a, vbyt, full + 8 * s);
+                    if (lane == 3 && vbyt) bulk_g2s(st + LY::VAL_BYTES, vb + p0a, vbyt, full + 8 * s);
+                    if (lane == 1 && cb) bulk_g2s(st + LY::OFF_COL, colidx + p0a, cb, full + 8 * s);
+                    if (lane == 2 && rb) bulk_g2s(st + LY::OFF_RP, rowptr + r0a, rb, full + 8 * s);
+                }
+            } else {
+                if (lane == 0) mbar_arrive(full + 8 * s);   // long row: consumers read global memory
+            }
+            if (++s == NSTG) { s = 0; ph ^= 1; }
+        }
+        return;
+    }
+    // ---------------------------------- consumers ----------------------------------
+    const int tid = threadIdx.x, w = tid >> 5;
+    const bool has_prev = MODE == 0 && vprev != nullptr;
+    const bool hints = l2_hints != 0;
+    const uint64_t pol_last = hints ? l2_policy_evict_last() : 0;
+    T d0 = (T)0, d1 = (T)0;
+    int tile = blockIdx.x;
+    int4 dn = make_int4(0, 0, 0, 0);
+    if (tile < nblk) dn = make_int4(rowblk[tile], rowblk[tile + 1], pblk[tile], pblk[tile + 1]);
+    for (; tile < nblk; tile += gridDim.x) {
+        const int r0 = dn.x, r1 = dn.y, p0 = dn.z, p1 = dn.w;
+        const int nt = tile + gridDim.x;
+        if (nt < nblk) dn = make_int4(rowblk[nt], rowblk[nt + 1], pblk[nt], pblk[nt + 1]);
+        const int nnzb = p1 - p0, nrows = r1 - r0;
+        mbar_wait(full + 8 * s, ph);
+        if (nnzb <= SP_NNZ) {
+            T* as = reinterpret_cast<T*>(smem + s * LY::STAGE);
+            T* bs = reinterpret_cast<T*>(smem + s * LY::STAGE + LY::VAL_BYTES);
+            const int32_t* cs = reinterpret_cast<const int32_t*>(smem + s * LY::STAGE + LY::OFF_COL);
+            const int32_t* rs = reinterpret_cast<const int32_t*>(smem + s * LY::STAGE + LY::OFF_RP);
+            const int p0a = p0 & ~3, r0a = r0 & ~3, off = p0 - p0a;
+            constexpr int U = SP_NNZ / SPP_CONS;
+            T xv[U];
+#pragma unroll
+            for (int u = 0; u < U; ++u) {
+                const int i = tid + u * SPP_CONS;
+                if (i < nnzb) xv[u] = __ldg(x + cs[off + i]);
+            }
+#pragma unroll
+            for (int u = 0; u < U; ++u) {
+                const int i = tid + u * SPP_CONS;
+                if (i < nnzb) {
+                    as[off + i] *= xv[u];
+                    bs[off + i] *= xv[u];
+                }
+            }
+            named_bar_sync(1, SPP_CONS);
+            const bool rp_staged = nrows <= SPP_RMAX;
+            for (int r = r0 + tid; r < r1; r += SPP_CONS) {
+                const T xr = want_dot ? __ldg(x + r) : (T)0;
+                const T vp = has_prev ? __ldg(vprev + r) : (T)0;
+                int a, b;
+                if (rp_staged) { a = rs[r - r0a]; b = rs[r + 1 - r0a]; }
+                else { a = rowptr[r]; b = rowptr[r + 1]; }
+                a -= p0a; b -= p0a;
+                T sa = (T)0, sb = (T)0;
+                for (int p = a; p < b; ++p) {
+                    sa += as[p];
+                    sb += bs[p];
+                }
+                pencil_row<T, MODE>(r, sa, sb, xr, vp, nrho, nbeta, has_prev, y0, y1, hints, pol_last, d0, d1);
+            }
+        } else {
+            double acca = 0.0, accb = 0.0;
+            for (int i = tid; i < nnzb; i += SPP_CONS) {
+                const T xv = __ldg(x + colidx[p0 + i]);
+                acca += (double)mul_rn<T>(va[p0 + i], xv);
+                accb += (double)mul_rn<T>(vb[p0 + i], xv);
+            }
+            acca = warp_sum(acca);
+            accb = warp_sum(accb);
+            if (lane == 0) {
+                red[w] = acca;
+                red[8 + w] = accb;
+            }
+            named_bar_sync(1, SPP_CONS);
+            if (tid == 0) {
+                double ta = 0.0, tb = 0.0;
+                for (int i = 0; i < SPP_CONS / 32; ++i) ta += red[i];
+                for (int i = 0; i < SPP_CONS / 32; ++i) tb += red[8 + i];
+                const T xr = want_dot ? x[r0] : (T)0;
+                const T vp = has_prev ? vprev[r0] : (T)0;
+                pencil_row<T, MODE>(r0, (T)ta, (T)tb, xr, vp, nrho, nbeta, has_prev, y0, y1, hints, pol_last, d0, d1);
+            }
+            named_bar_sync(1, SPP_CONS);
+        }
+        fence_proxy_async();   // generic-proxy writes to the stage precede its reuse by the TMA unit
+        __syncwarp();
+        if (lane == 0) mbar_arrive(empty + 8 * s);
+        if (++s == NSTG) { s = 0; ph ^= 1; }
+    }
+    if (want_dot) {
+        const double v0 = warp_sum((double)d0), v1 = warp_sum((double)d1);
+        if (lane == 0) {
+            red[w] = v0;
+            red[8 + w] = v1;
+        }
+        named_bar_sync(1, SPP_CONS);
+        if (tid == 0) {
+            double t0 = 0.0, t1 = 0.0;
+            for (int i = 0; i < SPP_CONS / 32; ++i) t0 += red[i];
+            for (int i = 0; i < SPP_CONS / 32; ++i) t1 += red[8 + i];
+            part[blockIdx.x] = t0;
+            part[gridDim.x + blockIdx.x] = t1;
+            __threadfence();
+            const unsigned t = atomicInc(ticket, gridDim.x - 1);
+            *flag = (t == gridDim.x - 1);
+        }
+        named_bar_sync(1, SPP_CONS);
+        if (*flag) {
+            __threadfence();
+            double a0 = 0.0, a1 = 0.0;
+            const volatile double* pv = part;
+            for (int g = tid; g < (int)gridDim.x; g += SPP_CONS) {
+                a0 += pv[g];
+                a1 += pv[gridDim.x + g];
+            }
+            a0 = warp_sum(a0);
+            a1 = warp_sum(a1);
+            named_bar_sync(1, SPP_CONS);
+            if (lane == 0) {
+                red[w] = a0;
+                red[8 + w] = a1;
+            }
+            named_bar_sync(1, SPP_CONS);
+            if (tid == 0) {
+                double t0 = 0.0, t1 = 0.0;
+                for (int i = 0; i < SPP_CONS / 32; ++i) t0 += red[i];
+                for (int i = 0; i < SPP_CONS / 32; ++i) t1 += red[8 + i];
+                out[0] = t0;
+                out[1] = t1;
+            }
+        }
+    }
+}
+
+__global__ void k_pattern_diff(const int32_t* __restrict__ a, const int32_t* __restrict__ b, int64_t n,
+                               int* __restrict__ diff) {
+    for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x)
+        if (a[i] != b[i]) {
+            *diff = 1;
+            return;
+        }
+}
+
 // SpMM for apply(A, ::Block) (blocklanczos.jl:38): the nonzero stream of a row block is staged ONCE (same TMA
 // ring as k_spmv_pipe) and used for all p <= 8 vectors of the block: 12*nnz + p*16n bytes instead of
 // p*(12*nnz + 16n).  Per vector the consumers do what k_spmv_pipe does — thread <-> nonzero gathers x_i and writes the
@@ -1513,6 +1766,9 @@ extern "C" int32_t b2k_op_create_transpose(b2k_ctx* ctx, b2k_op** out, const b2k
 // ------------------------------------------------------------------ apply ----
 
 static bool g_spmv_pipe = true;
+// L2 eviction hints of the fused pencil SpMV, on the terms of the chained single-operator step (basis.cu): on unless
+// B2K_L2_HINTS=0
+static bool g_pencil_l2_hints = true;
 extern "C" int32_t b2k_debug_set_onepass_variant(int32_t v);     // defined with the one-pass dense step below
 static int g_spmv_variant = 1;     // 1 (default): 2 stages x 4 CTAs/SM, 0: 3 stages x 3 CTAs/SM (B2K_SPMV_VARIANT)
 
@@ -1540,6 +1796,15 @@ int32_t b2k_spmv_init(b2k_ctx* ctx) {
                                        SppLayout<double, 2>::SMEM));
     B2K_CUDA(ctx, cudaFuncSetAttribute((k_spmv_pipe<float, 2, 4>), cudaFuncAttributeMaxDynamicSharedMemorySize,
                                        SppLayout<float, 2>::SMEM));
+#define PEN_ATTR(T, MODE)                                                                                      \
+    B2K_CUDA(ctx, cudaFuncSetAttribute((k_spmv_pencil<T, PEN_NSTG, PenCtas<T>::N, MODE>),                     \
+                                       cudaFuncAttributeMaxDynamicSharedMemorySize, PenLayout<T, PEN_NSTG>::SMEM))
+    PEN_ATTR(double, 0);
+    PEN_ATTR(double, 1);
+    PEN_ATTR(float, 0);
+    PEN_ATTR(float, 1);
+#undef PEN_ATTR
+    if (const char* e = getenv("B2K_L2_HINTS")) g_pencil_l2_hints = e[0] != '0';
     const char* sv = getenv("B2K_SPMV_VARIANT");
     if (sv) g_spmv_variant = atoi(sv) == 0 ? 0 : 1;
     const char* ov = getenv("B2K_ONEPASS_VARIANT");       // kernel of the flagged one-pass GKL step: 0 = A (default), 1 = B
@@ -1763,6 +2028,165 @@ extern "C" int32_t b2k_op_apply_adjoint(b2k_ctx* ctx, const b2k_op* op, b2k_vec 
                         (long long)rx.n, (long long)op->n_rows, (long long)ry.n, (long long)op->n_cols);
     return b2k_panel_project_dev(ctx, op->A, op->ld, op->n_rows, (int32_t)op->n_cols, rx, ry.ptr,
                                  rx.sharded);
+}
+
+// ------------------------------------------------------------------------------------------------
+// Pencils (A, B) for geneigsolve / Golub-Ye (golubye.jl).  A pencil is a host-side pairing: it owns no device memory,
+// and keeps A and B, which must outlive it.  Same-pattern CSR pairs take k_spmv_pencil (one launch per call), every
+// other pair the composition of b2k_op_apply / b2k_vec_axpby / b2k_vec_inner.
+
+struct b2k_pencil {
+    b2k_ctx* ctx;
+    const b2k_op* A;
+    const b2k_op* B;
+    int64_t n;
+    int32_t fused;
+};
+
+static int32_t g_pencil_path = 0;    // path of the last pencil call that passed its checks: 0 composed, 1 fused
+
+extern "C" int32_t b2k_debug_pencil_path(void) { return g_pencil_path; }
+
+extern "C" int32_t b2k_pencil_create(b2k_ctx* ctx, void** out, const b2k_op* A, const b2k_op* B) {
+    if (!ctx || !out || !A || !B) return B2K_EINVAL;
+    if (A == B) return b2k_fail(ctx, B2K_EINVAL, "pencil_create: A and B are the same operator");
+    for (const b2k_op* op : {A, B})
+        if (std::find(ctx->ops.begin(), ctx->ops.end(), op) == ctx->ops.end())
+            return b2k_fail(ctx, B2K_EINVAL, "pencil_create: an operator of another context");
+    if (ctx->nranks > 1) return b2k_fail(ctx, B2K_ENOTSUP, "pencil_create: row-sharded contexts are not supported");
+    if (A->n_rows != A->n_cols || B->n_rows != B->n_cols || A->n_rows != B->n_rows)
+        return b2k_fail(ctx, B2K_EDIM, "pencil_create: A (%lld x %lld) and B (%lld x %lld) must be square of one size",
+                        (long long)A->n_rows, (long long)A->n_cols, (long long)B->n_rows, (long long)B->n_cols);
+    int32_t fused = 0;
+    if (A->kind == 0 && B->kind == 0 && A->nnz == B->nnz && A->n_rows > 0) {
+        int* d_diff;
+        int h_diff = 0;
+        B2K_CUDA(ctx, B2K_DMALLOC(&d_diff, sizeof(int)));
+        B2K_CUDA(ctx, cudaMemsetAsync(d_diff, 0, sizeof(int), ctx->stream));
+        const int g = ctx->num_sms * 4;
+        k_pattern_diff<<<g, 256, 0, ctx->stream>>>(A->rowptr, B->rowptr, A->n_rows + 1, d_diff);
+        B2K_LAUNCH_CHECK(ctx);
+        if (A->nnz > 0) {
+            k_pattern_diff<<<g, 256, 0, ctx->stream>>>(A->colidx, B->colidx, A->nnz, d_diff);
+            B2K_LAUNCH_CHECK(ctx);
+        }
+        B2K_CUDA(ctx, cudaMemcpyAsync(&h_diff, d_diff, sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
+        B2K_TRY(b2k_stream_sync(ctx));
+        B2K_DFREE(d_diff);
+        fused = h_diff == 0;
+    }
+    *out = new b2k_pencil{ctx, A, B, A->n_rows, fused};
+    return B2K_OK;
+}
+
+extern "C" int32_t b2k_pencil_destroy(b2k_ctx* ctx, void* Pv) {
+    if (!ctx || !Pv) return B2K_EINVAL;
+    b2k_pencil* P = static_cast<b2k_pencil*>(Pv);
+    if (P->ctx != ctx) return b2k_fail(ctx, B2K_EINVAL, "pencil_destroy: the pencil belongs to another context");
+    delete P;
+    return B2K_OK;
+}
+
+// checks shared by both calls: resolves the handles (v[i] < 0 with opt[i]: absent), lengths, pairwise distinct
+static int32_t pencil_check(b2k_ctx* ctx, const b2k_pencil* P, const char* who, const b2k_vec* v, const bool* opt,
+                            int cnt, VecRef* r) {
+    if (P->ctx != ctx) return b2k_fail(ctx, B2K_EINVAL, "%s: the pencil belongs to another context", who);
+    if (ctx->nranks > 1) return b2k_fail(ctx, B2K_ENOTSUP, "%s: row-sharded contexts are not supported", who);
+    for (int i = 0; i < cnt; ++i) {
+        r[i].ptr = nullptr;
+        if (opt[i] && v[i] < 0) continue;
+        B2K_TRY(b2k_resolve(ctx, v[i], &r[i]));
+        if (r[i].n != P->n)
+            return b2k_fail(ctx, B2K_EDIM, "%s: vector %d has %lld entries, the pencil %lld", who, i,
+                            (long long)r[i].n, (long long)P->n);
+        for (int j = 0; j < i; ++j)
+            if (r[j].ptr && r[j].ptr == r[i].ptr)
+                return b2k_fail(ctx, B2K_EINVAL, "%s: vectors %d and %d are the same", who, j, i);
+    }
+    return B2K_OK;
+}
+
+template <typename T, int MODE>
+static int32_t pencil_launch(b2k_ctx* ctx, const b2k_pencil* P, const VecRef& x, const VecRef& y0, const VecRef& y1,
+                             double rho, const VecRef* vprev, double beta, bool want_dot, double bytes) {
+    const b2k_op* A = P->A;
+    const int grid = std::min(A->nblk, PenCtas<T>::N * ctx->num_sms);
+    const int pr = b2k_prof_begin(ctx, 0, bytes);
+    k_spmv_pencil<T, PEN_NSTG, PenCtas<T>::N, MODE><<<grid, SPP_THREADS, PenLayout<T, PEN_NSTG>::SMEM, ctx->stream>>>(
+        A->rowptr, A->colidx, (const T*)A->vals, (const T*)P->B->vals, (const T*)x.ptr, (T*)y0.ptr, (T*)y1.ptr,
+        A->rowblk, A->pblk, A->nblk, (T)(-rho), vprev ? (const T*)vprev->ptr : nullptr, (T)(-beta), want_dot ? 1 : 0,
+        g_pencil_l2_hints ? 1 : 0, ctx->d_part_s, ctx->d_sync, ctx->d_res);
+    b2k_prof_end(ctx, pr);
+    B2K_LAUNCH_CHECK(ctx);
+    return B2K_OK;
+}
+
+extern "C" int32_t b2k_pencil_apply(b2k_ctx* ctx, const void* Pv, b2k_vec x, b2k_vec w, b2k_vec bx, double rho,
+                                    b2k_vec vprev, double beta, double* dot) {
+    if (!ctx || !Pv) return B2K_EINVAL;
+    const b2k_pencil* P = static_cast<const b2k_pencil*>(Pv);
+    const b2k_vec v[4] = {x, w, bx, vprev};
+    const bool opt[4] = {false, false, false, true};
+    VecRef r[4];
+    B2K_TRY(pencil_check(ctx, P, "pencil_apply", v, opt, 4, r));
+    const bool has_prev = r[3].ptr != nullptr;
+    g_pencil_path = P->fused;
+    if (!P->fused) {
+        B2K_TRY(b2k_op_apply(ctx, P->A, x, w));
+        B2K_TRY(b2k_op_apply(ctx, P->B, x, bx));
+        B2K_TRY(b2k_vec_axpby(ctx, w, bx, -rho, 1.0));
+        if (has_prev) B2K_TRY(b2k_vec_axpby(ctx, w, vprev, -beta, 1.0));
+        return dot ? b2k_vec_inner(ctx, x, w, dot) : B2K_OK;
+    }
+    if (P->n == 0) {
+        if (dot) *dot = 0.0;
+        return B2K_OK;
+    }
+    const double es = ctx->esize, n = (double)P->n;
+    const double bytes = (double)P->A->nnz * (2 * es + 4) + 4.0 * (n + 1) + (has_prev ? 4.0 : 3.0) * es * n;
+    if (ctx->dtype == B2K_F64)
+        B2K_TRY((pencil_launch<double, 0>(ctx, P, r[0], r[1], r[2], rho, has_prev ? &r[3] : nullptr, beta, dot, bytes)));
+    else
+        B2K_TRY((pencil_launch<float, 0>(ctx, P, r[0], r[1], r[2], rho, has_prev ? &r[3] : nullptr, beta, dot, bytes)));
+    if (!dot) return B2K_OK;
+    B2K_TRY(b2k_fetch_results(ctx, 1, 0));
+    *dot = ctx->h_res[0];
+    return B2K_OK;
+}
+
+extern "C" int32_t b2k_pencil_rayleigh(b2k_ctx* ctx, const void* Pv, b2k_vec x, b2k_vec ax, b2k_vec bx,
+                                       double* xax, double* xbx) {
+    if (!ctx || !Pv) return B2K_EINVAL;
+    const b2k_pencil* P = static_cast<const b2k_pencil*>(Pv);
+    const b2k_vec v[3] = {x, ax, bx};
+    const bool opt[3] = {false, false, false};
+    VecRef r[3];
+    B2K_TRY(pencil_check(ctx, P, "pencil_rayleigh", v, opt, 3, r));
+    g_pencil_path = P->fused;
+    const bool want_dot = xax || xbx;
+    if (!P->fused) {
+        B2K_TRY(b2k_op_apply(ctx, P->A, x, ax));
+        B2K_TRY(b2k_op_apply(ctx, P->B, x, bx));
+        if (xax) B2K_TRY(b2k_vec_inner(ctx, x, ax, xax));
+        if (xbx) B2K_TRY(b2k_vec_inner(ctx, x, bx, xbx));
+        return B2K_OK;
+    }
+    if (P->n == 0) {
+        if (xax) *xax = 0.0;
+        if (xbx) *xbx = 0.0;
+        return B2K_OK;
+    }
+    const double es = ctx->esize, n = (double)P->n;
+    const double bytes = (double)P->A->nnz * (2 * es + 4) + 4.0 * (n + 1) + 3.0 * es * n;
+    if (ctx->dtype == B2K_F64)
+        B2K_TRY((pencil_launch<double, 1>(ctx, P, r[0], r[1], r[2], 0.0, nullptr, 0.0, want_dot, bytes)));
+    else
+        B2K_TRY((pencil_launch<float, 1>(ctx, P, r[0], r[1], r[2], 0.0, nullptr, 0.0, want_dot, bytes)));
+    if (!want_dot) return B2K_OK;
+    B2K_TRY(b2k_fetch_results(ctx, 2, 0));
+    if (xax) *xax = ctx->h_res[0];
+    if (xbx) *xbx = ctx->h_res[1];
+    return B2K_OK;
 }
 
 // ------------------------------------------------------------------------------------------------

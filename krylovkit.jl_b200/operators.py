@@ -199,6 +199,61 @@ def apply(op, x: B200Vec, a0: float = 0.0, a1: float = 1.0) -> B200Vec:
     return y
 
 
+class B200Pencil:
+    """The pencil (A, B) of a generalized eigenproblem A x = λ B x (geneigsolve): b2k_pencil_*.  A and B are square
+    device operators of one context and one size; the pencil holds references to both.  Same-pattern CSR pairs (an
+    assembled stencil pair, a stiffness / mass pair of one mesh) are applied by one fused pass over both matrices,
+    every other pair by the composition of separate applies; both give the same bits for the vectors.  Calling the
+    pencil on x returns (A x, B x): KrylovKit's `genapply(f, x) = f(x)` (apply.jl:23)."""
+
+    def __init__(self, A: B200Operator, B: B200Operator):
+        if A.ctx is not B.ctx:
+            raise ValueError("B200Pencil: A and B must belong to one context")
+        ctx = A.ctx
+        h = C.c_void_p()
+        ctx.check(ctx.lib.b2k_pencil_create(ctx.h, C.byref(h), A.h, B.h))
+        self.ctx, self.A, self.B, self.h = ctx, A, B, h
+        self._fin = weakref.finalize(self, _destroy_pencil, ctx.lib, ctx.h, h, ctx._alive)
+
+    def free(self):
+        self._fin()
+
+    def apply_into(self, x: B200Vec, w: B200Vec, bx: B200Vec, rho: float, vprev: B200Vec | None = None,
+                   beta: float = 0.0, dot: bool = False):
+        """bx = B x, w = add!!(A x, bx, -ρ) [then add!!(w, vprev, -β)] — golubye.jl:198-202; returns <x, w> when `dot`
+        (b2k_pencil_apply)."""
+        out = C.c_double()
+        self.ctx.check(self.ctx.lib.b2k_pencil_apply(self.ctx.h, self.h, x.handle, w.handle, bx.handle, float(rho),
+                                                     -1 if vprev is None else vprev.handle, float(beta),
+                                                     C.byref(out) if dot else None))
+        return out.value if dot else None
+
+    def rayleigh_into(self, x: B200Vec, ax: B200Vec, bx: B200Vec, dots: bool = True):
+        """ax = A x, bx = B x and, when `dots`, (<x, ax>, <x, bx>) from the same pass (b2k_pencil_rayleigh)."""
+        a, b = C.c_double(), C.c_double()
+        self.ctx.check(self.ctx.lib.b2k_pencil_rayleigh(self.ctx.h, self.h, x.handle, ax.handle, bx.handle,
+                                                        C.byref(a) if dots else None, C.byref(b) if dots else None))
+        return (a.value, b.value) if dots else None
+
+    def __call__(self, x: B200Vec):
+        ax, bx = x.ctx.empty(x.space), x.ctx.empty(x.space)
+        self.rayleigh_into(x, ax, bx, dots=False)
+        return ax, bx
+
+
+def _destroy_pencil(lib, ctx_h, h, alive):
+    if alive[0]:
+        lib.b2k_pencil_destroy(ctx_h, h)
+
+
+def genapply(f, x: B200Vec):
+    """genapply — src/apply.jl:22-23: (apply(A, x), apply(B, x)) for a tuple (A, B) of operators or callables,
+    f(x) -> (A x, B x) for a callable; a B200Pencil forms both products in one call."""
+    if isinstance(f, tuple):
+        return apply(f[0], x), apply(f[1], x)
+    return f(x)
+
+
 def apply_normal(op, x: B200Vec) -> B200Vec:
     """apply_normal — src/apply.jl:14,16,18."""
     if isinstance(op, B200Operator):
