@@ -30,7 +30,8 @@ k_phase(const __grid_constant__ PhaseParams<T> p, const __grid_constant__ ColLis
     pipe_setup(sm, ragged);
     Pipe st;
     if (threadIdx.x >= NCONS) producer_phase<T>(p, cl, sm, st);
-    else consumer_phase<T, UPDATE, PROJECT>(p, sm, st);
+    else if (p.prologue) consumer_phase<T, UPDATE, PROJECT, true>(p, sm, st);
+    else consumer_phase<T, UPDATE, PROJECT, false>(p, sm, st);
 }
 
 // Cooperative fused Gram-Schmidt kernel: up to three phases in one launch, separated by
@@ -40,6 +41,7 @@ struct FusedParams {
     PhaseParams<T> ph[3];
     int32_t kind[3];
     int32_t nph;
+    int32_t run_ahead[2];    // boundary i (after phase i): producers skip it (boundary_sync), set by launch_fused
     unsigned* barrier;
     unsigned barrier_base;   // counter value before this launch
     const int* stop;         // device flag: when set, the launch does nothing (see FinalizeParams)
@@ -53,17 +55,19 @@ struct FusedParams {
 // fixed order as on one GPU) and stores them into EVERY rank's window; every CTA of every rank then waits, in
 // its own window, for the nranks contributions — which also proves that all local CTAs have arrived.  One
 // NVLink store latency instead of a kernel boundary + ncclAllReduce + a kernel boundary.
+// Like grid_barrier, called by the consumer threads only when the boundary is run-ahead.
 template <typename T>
 __device__ __forceinline__ void peer_boundary(const FusedParams<T>& fp, int i, uint8_t* smem) {
+    const bool ra = fp.run_ahead[i] != 0;
     __threadfence();
-    asm volatile("fence.proxy.async;" ::: "memory");
-    __syncthreads();
+    if (!ra) asm volatile("fence.proxy.async;" ::: "memory");
+    boundary_sync(ra);
     int* flag = reinterpret_cast<int*>(smem + OFF_RED + 256);
     if (threadIdx.x == 0) {
         const unsigned old = atomicAdd(fp.barrier, 1u);
         *flag = (old == fp.barrier_base + (unsigned)(i + 1) * gridDim.x - 1u);
     }
-    __syncthreads();
+    boundary_sync(ra);
     const PeerDev& pd = fp.ps.pd;
     const int tid = threadIdx.x;
     if (fp.ph[i].part_h == nullptr) {
@@ -76,7 +80,7 @@ __device__ __forceinline__ void peer_boundary(const FusedParams<T>& fp, int i, u
             if (tid == 0) peer_publish1(pd, PEER_CH_NORM, sq, a);
         }
         peer_wait(pd, PEER_CH_NORM, sq, tid);
-        __syncthreads();
+        boundary_sync(ra);
         return;
     }
     const unsigned long long seq = fp.ps.seq_coef[i];
@@ -94,7 +98,7 @@ __device__ __forceinline__ void peer_boundary(const FusedParams<T>& fp, int i, u
         if (tid < pd.nranks) st_release_sys_u64(peer_flag(pd, tid, PEER_CH_COEF, seq, pd.rank), seq);
     }
     peer_wait(pd, PEER_CH_COEF, seq, tid);
-    __syncthreads();
+    boundary_sync(ra);
 }
 
 template <typename T>
@@ -126,14 +130,22 @@ k_gs_fused(const __grid_constant__ FusedParams<T> fp, const __grid_constant__ Co
         if (prod) {
             producer_phase<T>(fp.ph[i], cl, sm, st);
         } else {
-            if (fp.kind[i] == 0) consumer_phase<T, false, true>(fp.ph[i], sm, st);
-            else if (fp.kind[i] == 1) consumer_phase<T, true, true>(fp.ph[i], sm, st);
-            else consumer_phase<T, true, false>(fp.ph[i], sm, st);
+            const PhaseParams<T>& p = fp.ph[i];
+            if (fp.kind[i] == 0) {
+                if (p.prologue) consumer_phase<T, false, true, true>(p, sm, st);
+                else consumer_phase<T, false, true, false>(p, sm, st);
+            } else if (fp.kind[i] == 1) {
+                if (p.prologue) consumer_phase<T, true, true, true>(p, sm, st);
+                else consumer_phase<T, true, true, false>(p, sm, st);
+            } else {
+                if (p.prologue) consumer_phase<T, true, false, true>(p, sm, st);
+                else consumer_phase<T, true, false, false>(p, sm, st);
+            }
         }
         if (tr0) b2k_trace(fp.trace, 12 + i);           // CTA 0 has finished the phase's tiles
-        if (i + 1 < fp.nph) {
+        if (i + 1 < fp.nph && !(prod && fp.run_ahead[i])) {
             if (fp.ps.on) peer_boundary<T>(fp, i, smem);
-            else grid_barrier(fp.barrier, fp.barrier_base + (unsigned)(i + 1) * gridDim.x);
+            else grid_barrier(fp.barrier, fp.barrier_base + (unsigned)(i + 1) * gridDim.x, fp.run_ahead[i] != 0);
             if (tr0) b2k_trace(fp.trace, 15 + i);       // ... and left the boundary
         }
     }
@@ -1075,8 +1087,29 @@ int grid_for_rows(const b2k_ctx* ctx, int64_t n) {
 
 bool g_coop_launch = true;   // B2K_COOP_LAUNCH=0: plain launch of the fused sweep (measurement only: no co-residency guarantee)
 
+// Does phase `st` store into a vector that phase `rd` streams (its x or one of its panel columns)?
+template <typename T>
+bool stores_into_stream(const PhaseParams<T>& st, const PhaseParams<T>& rd, const ColList& cl) {
+    if (!st.store_x || !st.xout) return false;
+    const T* lo = st.xout;
+    const T* hi = st.xout + st.n;
+    auto hits = [&](const T* v) { return v && v < hi && lo < v + rd.n; };
+    if (hits(rd.x)) return true;
+    for (int m = 0; m < rd.k; ++m)
+        if (hits(rd.base + (int64_t)cl.c[m] * rd.ld)) return true;
+    return false;
+}
+
 template <typename T>
 int32_t launch_fused(b2k_ctx* ctx, FusedParams<T>& fp, const ColList& cl, int grid) {
+    // Producers may run through boundary i into phase i + 1 unless a phase up to i stored into a vector phase
+    // i + 1 streams: a bulk copy issued before the boundary's fence.proxy.async could read a row its store has
+    // not yet reached.
+    for (int i = 0; i + 1 < fp.nph; ++i) {
+        bool ra = true;
+        for (int j = 0; j <= i; ++j) ra = ra && !stores_into_stream<T>(fp.ph[j], fp.ph[i + 1], cl);
+        fp.run_ahead[i] = ra ? 1 : 0;
+    }
     // the barrier counter only ever increases; wrap-around is handled by the signed compare
     fp.barrier = ctx->d_sync + 1;
     fp.barrier_base = ctx->barrier_base;
@@ -1136,6 +1169,13 @@ void fill_cols(ColList& cl, const std::vector<int32_t>& idx, int off, int cnt) {
     for (int i = 0; i < cnt; ++i) cl.c[i] = idx[off + i];
 }
 
+// Column list of a Lanczos step's sweeps.  With the three-term prologue (PhaseParams::prologue) it is rotated by
+// two, [v_prev, v, q_0, ..., q_{K1-3}], so that the prologue's operands are the first chunk of every tile.
+void lanczos_cols(ColList& cl, const Panel& pn, int K1, bool prologue) {
+    const int rot = prologue ? 2 : 0;
+    for (int i = 0; i < K1; ++i) cl.c[(i + rot) % K1] = pn.idx[i];
+}
+
 template <typename T>
 PhaseParams<T> base_params(const Panel& pn, int k, const void* x, void* xout) {
     PhaseParams<T> p;
@@ -1146,7 +1186,6 @@ PhaseParams<T> base_params(const Panel& pn, int k, const void* x, void* xout) {
     p.k = k;
     p.x = (const T*)x;
     p.xout = (T*)xout;
-    p.nvec = 1;
     p.beta_mode = 1;
     p.betax = (T)1;
     p.alphac = (T)1;
@@ -1653,21 +1692,22 @@ extern "C" int32_t b2k_lanczos_expand(b2k_ctx* ctx, const b2k_op* op, const b2k_
             if (fusable) {
                 const int grid = f64 ? grid_for_rows<double>(ctx, pn.n) : grid_for_rows<float>(ctx, pn.n);
                 ColList cl;
-                for (int i = 0; i < K1; ++i) cl.c[i] = pn.idx[i];
+                lanczos_cols(cl, pn, K1, prologue);
                 double* PA = b2k_part_set(ctx, 0);
                 double* PN = b2k_part_set(ctx, 2);
 #define BUILD_AND_LAUNCH(T)                                                                   \
     {                                                                                         \
         FusedParams<T> fp;                                                                    \
         memset(&fp, 0, sizeof(fp));                                                           \
-        PhaseParams<T> a = base_params<T>(pn, K1, rw.ptr, rw.ptr);                            \
+        PhaseParams<T> a = base_params<T>(pn, K1, rw.ptr, nullptr);                           \
+        PhaseParams<T> c = base_params<T>(pn, K1, rw.ptr, rw.ptr);                            \
         if (prologue) {                                                                       \
-            a.nvec = 3; a.e1 = (const T*)vprev.ptr; a.e2 = (const T*)rv.ptr;                  \
-            a.c1 = (T)(-beta_old); a.c2 = (T)(-alpha); a.store_x = 1;                         \
-            if (defer_alpha) a.c2_dev = ctx->d_res + S_A0;                                    \
+            for (PhaseParams<T>* q : {&a, &c}) {                                              \
+                q->prologue = 1; q->c1 = (T)(-beta_old); q->c2 = (T)(-alpha);                 \
+                if (defer_alpha) q->c2_dev = ctx->d_res + S_A0;                               \
+            }                                                                                 \
         }                                                                                     \
         a.part_h = PA;                                                                        \
-        PhaseParams<T> c = base_params<T>(pn, K1, rw.ptr, rw.ptr);                            \
         c.store_x = 1; c.coef = PA; c.coef_sets = grid; c.coef_stride = B2K_KSTRIDE;          \
         c.alphac = (T)-1; c.part_n = PN;                                                      \
         fp.ph[0] = a; fp.kind[0] = 0; fp.ph[1] = c; fp.kind[1] = 2; fp.nph = 2;               \
@@ -1689,23 +1729,24 @@ extern "C" int32_t b2k_lanczos_expand(b2k_ctx* ctx, const b2k_op* op, const b2k_
                 // sweep, the all-reduce of the coefficients sits where the grid barrier was
                 const int grid = f64 ? grid_for_rows<double>(ctx, pn.n) : grid_for_rows<float>(ctx, pn.n);
                 ColList cl;
-                for (int i = 0; i < K1; ++i) cl.c[i] = pn.idx[i];
+                lanczos_cols(cl, pn, K1, prologue);
                 double* PA = b2k_part_set(ctx, 0);
                 double* PN = b2k_part_set(ctx, 2);
 #define SPLIT_SWEEPS(T)                                                                       \
     {                                                                                         \
-        PhaseParams<T> a = base_params<T>(pn, K1, rw.ptr, rw.ptr);                            \
+        PhaseParams<T> a = base_params<T>(pn, K1, rw.ptr, nullptr);                           \
+        PhaseParams<T> c = base_params<T>(pn, K1, rw.ptr, rw.ptr);                            \
         if (prologue) {                                                                       \
-            a.nvec = 3; a.e1 = (const T*)vprev.ptr; a.e2 = (const T*)rv.ptr;                  \
-            a.c1 = (T)(-beta_old); a.c2 = (T)(-alpha); a.store_x = 1;                         \
-            if (defer_alpha) a.c2_dev = ctx->d_res + S_A0;                                    \
+            for (PhaseParams<T>* q : {&a, &c}) {                                              \
+                q->prologue = 1; q->c1 = (T)(-beta_old); q->c2 = (T)(-alpha);                 \
+                if (defer_alpha) q->c2_dev = ctx->d_res + S_A0;                               \
+            }                                                                                 \
         }                                                                                     \
         a.part_h = PA;                                                                        \
         const int pr = b2k_prof_begin(ctx, 1, (2.0 * K1 + 3.0) * sizeof(T) * (double)pn.n);   \
         B2K_TRY(launch_phase<T>(ctx, a, cl, 0, grid));                                        \
         B2K_TRY(enqueue_finalize(ctx, PA, nullptr, nullptr, grid, K1, S_H, S_N));             \
         B2K_TRY(b2k_allreduce(ctx, ctx->d_res + S_H, K1, pn.sharded));                        \
-        PhaseParams<T> c = base_params<T>(pn, K1, rw.ptr, rw.ptr);                            \
         c.store_x = 1; c.coef = ctx->d_res + S_H; c.coef_sets = 1; c.coef_stride = 0;         \
         c.alphac = (T)-1; c.part_n = PN;                                                      \
         B2K_TRY(launch_phase<T>(ctx, c, cl, 2, grid));                                        \
@@ -1837,17 +1878,19 @@ int32_t chain_step_gs(b2k_ctx* ctx, const Panel& pn, int K1, const VecRef& rw, c
                       bool scale_after) {
     const int grid = grid_for_rows<T>(ctx, pn.n);
     ColList cl;
-    for (int i = 0; i < K1; ++i) cl.c[i] = pn.idx[i];
+    lanczos_cols(cl, pn, K1, true);
     double* PA = b2k_part_set(ctx, 0);
     double* PN = b2k_part_set(ctx, 2);
     FusedParams<T> fp;
     memset(&fp, 0, sizeof(fp));
-    PhaseParams<T> a = base_params<T>(pn, K1, rw.ptr, rw.ptr);
-    a.nvec = 3; a.e1 = (const T*)vprev.ptr; a.e2 = (const T*)rv.ptr; a.store_x = 1;
-    a.c1_dev = rec_prev + 2;          // beta of the previous step
-    a.c2_dev = rec + 0;               // <v, A v> of this step
-    a.part_h = PA;
+    PhaseParams<T> a = base_params<T>(pn, K1, rw.ptr, nullptr);
     PhaseParams<T> c = base_params<T>(pn, K1, rw.ptr, rw.ptr);
+    for (PhaseParams<T>* q : {&a, &c}) {
+        q->prologue = 1;
+        q->c1_dev = rec_prev + 2;     // beta of the previous step
+        q->c2_dev = rec + 0;          // <v, A v> of this step
+    }
+    a.part_h = PA;
     c.store_x = 1; c.coef = PA; c.coef_sets = grid; c.coef_stride = B2K_KSTRIDE;
     c.alphac = (T)-1; c.part_n = PN;
     fp.ph[0] = a; fp.kind[0] = 0; fp.ph[1] = c; fp.kind[1] = 2; fp.nph = 2;
@@ -1874,9 +1917,11 @@ int32_t chain_step_gs(b2k_ctx* ctx, const Panel& pn, int K1, const VecRef& rw, c
             return reinterpret_cast<double*>(win + PEER_OFF_SLOTS) + (size_t)((ch * 2 + (int)(seq & 1ull)) * PEER_MAXR) * PEER_SLOT;
         };
         // <v, A v>: the per-rank partials the SpMV published (rank order)
-        fp.ph[0].c2_dev = slot(PEER_CH_ALPHA, ps.seq_alpha);
-        fp.ph[0].c2_sets = ps.pd.nranks;
-        fp.ph[0].c2_stride = PEER_SLOT;
+        for (int i = 0; i < 2; ++i) {
+            fp.ph[i].c2_dev = slot(PEER_CH_ALPHA, ps.seq_alpha);
+            fp.ph[i].c2_sets = ps.pd.nranks;
+            fp.ph[i].c2_stride = PEER_SLOT;
+        }
         // projection coefficients: the per-rank sums in my window instead of the per-CTA partials
         fp.ph[1].coef = slot(PEER_CH_COEF, ps.seq_coef[0]);
         fp.ph[1].coef_sets = ps.pd.nranks;

@@ -13,8 +13,9 @@
 //     C = 8 for f64, 16 for f32); NS = 12 slots form the ring, each with a full/empty
 //     mbarrier pair; the producer's lanes issue one 1-D bulk copy per column (2 KB f64),
 //     so arbitrary (non-contiguous) column handle lists cost nothing extra;
-//   * the vector being orthogonalised rides in a separate 3-deep ring ("w slots") that
-//     can also carry the two extra vectors of the Lanczos three-term prologue;
+//   * the vector being orthogonalised rides in a separate 3-deep ring ("w slots"); the two
+//     extra vectors of the Lanczos three-term prologue are basis columns and ride in the
+//     panel ring's first chunk (PhaseParams::prologue);
 //   * UPDATE phases map thread <-> row (sequential fma over the columns: the same
 //     association as the reference's chain of add!! calls, orthonormal.jl:146-148);
 //     PROJECT phases map warp <-> column, lane <-> rows (128-bit LDS), accumulators in
@@ -77,8 +78,11 @@ struct PhaseParams {
     // the streamed vector
     const T* x;
     T* xout;         // may be nullptr
-    const T* e1;     // prologue vectors (nvec == 3): x' = (x + c1*e1) + c2*e2
-    const T* e2;
+    // Lanczos three-term prologue: x' = (x + c1*v_prev) + c2*v.  v_prev and v are the last two basis columns;
+    // the host lists the columns rotated by two, [v_prev, v, q_0, ..., q_{k-3}], so both arrive with the first
+    // chunk of every tile and are read from the ring once for the prologue and the projection (or update) alike.
+    // Coefficients and partials keep the original column index.
+    int32_t prologue;
     T c1, c2;
     const double* c1_dev;   // if set: c1 = -(*c1_dev)  (beta of the previous step, kept on the device)
     const double* c2_dev;   // if set: c2 = -(*c2_dev), a device scalar produced by the previous kernel
@@ -97,8 +101,7 @@ struct PhaseParams {
     const double* scale_norm;
     int32_t scale_G, scale_stride;
     double scale_tol;
-    int32_t nvec;    // 1 or 3
-    int32_t store_x; // write x'' (UPDATE) or x' (prologue write-back) to xout
+    int32_t store_x; // write x'' (UPDATE) to xout
     int32_t l2_hints; // panel loads evict_first, the stored vector evict_last (common.cuh)
     // UPDATE: x'' = betax*x' + sum_j Q[:,j]*cs[j],  cs[j] = alphac * sum_g coef[g*stride+j]
     const double* coef;
@@ -207,15 +210,12 @@ __device__ __forceinline__ void producer_phase(const PhaseParams<T>& p, const Co
         const int64_t r0 = tile * R;
         const int rt = (int)((p.n - r0) < R ? (p.n - r0) : R);
         const uint32_t bytes = (uint32_t)((rt * sizeof(T) + 15) & ~(size_t)15);
-        // the vector tile (+ prologue vectors): producer warp 0
+        // the vector tile: producer warp 0
         if (me == 0) {
             mbar_wait(sm.wempty + 8 * st.ws, st.wph ^ 1);
-            if (lane == 0) mbar_expect_tx(sm.wfull + 8 * st.ws, bytes * (uint32_t)p.nvec);
-            __syncwarp();
-            if (lane < p.nvec) {
-                const T* src = (lane == 0) ? p.x : (lane == 1 ? p.e1 : p.e2);
-                bulk_g2s(sm.wring + st.ws * (3 * R * (int)sizeof(T)) + lane * R * (int)sizeof(T),
-                         src + r0, bytes, sm.wfull + 8 * st.ws);
+            if (lane == 0) {
+                mbar_expect_tx(sm.wfull + 8 * st.ws, bytes);
+                bulk_g2s(sm.wring + st.ws * WSLOT_MAX, p.x + r0, bytes, sm.wfull + 8 * st.ws);
             }
         }
         if (++st.ws == NW) { st.ws = 0; st.wph ^= 1; }
@@ -260,7 +260,9 @@ template <> struct VecOps<float> {
     }
 };
 
-template <typename T, bool UPDATE, bool PROJECT>
+// PRO: the Lanczos three-term prologue (PhaseParams::prologue).  A template parameter, so that the sweeps without it
+// compile to exactly the code they had before the prologue moved into the panel ring.
+template <typename T, bool UPDATE, bool PROJECT, bool PRO>
 __device__ __forceinline__ void consumer_phase(const PhaseParams<T>& p, const SmemView& sm,
                                                Pipe& st) {
     using CF = Cfg<T>;
@@ -275,17 +277,17 @@ __device__ __forceinline__ void consumer_phase(const PhaseParams<T>& p, const Sm
     T* cs = reinterpret_cast<T*>(sm.raw + OFF_CS);
     T* w1 = reinterpret_cast<T*>(sm.raw + OFF_W1);
     double* red = reinterpret_cast<double*>(sm.raw + OFF_RED);
-
     if (UPDATE) {
-        // every CTA reduces the previous phase's partials itself (fixed order, see coef_colsum)
+        // every CTA reduces the previous phase's partials itself (fixed order, see coef_colsum); cs is kept in
+        // ring order
         if (p.coef_t) {
-            for (int j = tid; j < p.k; j += NCONS) cs[j] = p.alphac * p.coef_t[j];
+            for (int j = tid; j < p.k; j += NCONS) cs[PRO ? (j + 2) % p.k : j] = p.alphac * p.coef_t[j];
         } else {
             const int L = coef_lanes(p.k);
             const int j = tid / L, l = tid % L;
             const bool valid = j < p.k;
             const double h = coef_colsum(p.coef, p.coef_sets, p.coef_stride, j, l, L, valid);
-            if (valid && l == 0) cs[j] = p.alphac * (T)h;
+            if (valid && l == 0) cs[PRO ? (j + 2) % p.k : j] = p.alphac * (T)h;
         }
         named_bar_sync(1, NCONS);
     }
@@ -333,11 +335,17 @@ __device__ __forceinline__ void consumer_phase(const PhaseParams<T>& p, const Sm
         const int64_t r0 = tile * R;
         const int rt = (int)((p.n - r0) < R ? (p.n - r0) : R);
         mbar_wait(sm.wfull + 8 * st.ws, st.wph);
-        const T* wv = reinterpret_cast<const T*>(sm.raw + OFF_WRING) + st.ws * 3 * R;
+        const T* wv = reinterpret_cast<const T*>(sm.raw + OFF_WRING + st.ws * WSLOT_MAX);
         T xv = wv[tid];
-        if (p.nvec == 3) {
-            xv = fma(c1, wv[R + tid], xv);
-            xv = fma(c2, wv[2 * R + tid], xv);
+        T vprev = (T)0, vcur = (T)0;
+        if (PRO) {
+            // v_prev and v are the first two columns of the tile's first chunk
+            mbar_wait(sm.full + 8 * st.s, st.ph);
+            const T* slot = reinterpret_cast<const T*>(sm.raw + OFF_RING + st.s * SLOT_BYTES);
+            vprev = slot[tid];
+            vcur = slot[R + tid];
+            xv = fma(c1, vprev, xv);
+            xv = fma(c2, vcur, xv);
         }
         if (tid >= rt) xv = (T)0;
         T acc = xv;
@@ -348,7 +356,8 @@ __device__ __forceinline__ void consumer_phase(const PhaseParams<T>& p, const Sm
                 mbar_wait(sm.full + 8 * st.s, st.ph);
                 const T* slot = reinterpret_cast<const T*>(sm.raw + OFF_RING + st.s * SLOT_BYTES);
                 const int ncol = (p.k - c * C) < C ? (p.k - c * C) : C;
-                if (ncol == C) {
+                const int j0 = (PRO && c == 0) ? 2 : 0;    // v_prev and v are added last, in original column order
+                if (ncol == C && j0 == 0) {
                     T cv[C];
 #pragma unroll
                     for (int i = 0; i < C / VEC; ++i)
@@ -356,13 +365,17 @@ __device__ __forceinline__ void consumer_phase(const PhaseParams<T>& p, const Sm
 #pragma unroll
                     for (int jj = 0; jj < C; ++jj) acc = fma(slot[jj * R + tid], cv[jj], acc);
                 } else {
-                    for (int jj = 0; jj < ncol; ++jj) acc = fma(slot[jj * R + tid], cs[c * C + jj], acc);
+                    for (int jj = j0; jj < ncol; ++jj) acc = fma(slot[jj * R + tid], cs[c * C + jj], acc);
                 }
                 if (!PROJECT) {
                     __syncwarp();
                     if (lane == 0) mbar_arrive(sm.empty + 8 * st.s);
                 }
                 if (++st.s == NS) { st.s = 0; st.ph ^= 1; }
+            }
+            if (PRO) {
+                acc = fma(vprev, cs[0], acc);
+                acc = fma(vcur, cs[1], acc);
             }
             if (tid >= rt) acc = (T)0;
         }
@@ -420,10 +433,10 @@ __device__ __forceinline__ void consumer_phase(const PhaseParams<T>& p, const Sm
         for (int c = 0; c < MAXCH; ++c) {
 #pragma unroll
             for (int cc = 0; cc < CPW; ++cc) {
-                const int j = c * C + cc * 8 + w;
+                const int j = c * C + cc * 8 + w;            // ring position
                 double v = warp_sum((double)acc_h[c][cc]);   // warp-uniform branch below
                 if (c < nch && j < p.k && lane == 0)
-                    p.part_h[(size_t)blockIdx.x * B2K_KSTRIDE + j] = v;
+                    p.part_h[(size_t)blockIdx.x * B2K_KSTRIDE + (PRO ? (j < 2 ? j + p.k - 2 : j - 2) : j)] = v;
             }
         }
     }
@@ -525,19 +538,29 @@ __device__ __forceinline__ void finalize_block(const FinalizeParams& f, int tid,
     }
 }
 
+// Barrier among the CTA's threads at a phase boundary.  run_ahead: only the NCONS consumer threads take part
+// (named barrier 1) and the producer warps go straight on filling the ring with the next phase's tiles — allowed
+// only when no earlier phase stored into a vector the next phase streams (launch_fused decides).  Otherwise all
+// threads, so that no bulk copy of the next phase is issued before every CTA's stores are visible to it.
+__device__ __forceinline__ void boundary_sync(bool run_ahead) {
+    if (run_ahead) named_bar_sync(1, NCONS);
+    else __syncthreads();
+}
+
 // grid-wide barrier for the cooperative fused kernel.  `target` is the value the
-// monotonically increasing counter reaches when every CTA has arrived.
-__device__ __forceinline__ void grid_barrier(unsigned* counter, unsigned target) {
+// monotonically increasing counter reaches when every CTA has arrived.  Called by every thread of the CTA, or by
+// the consumer threads only when run_ahead (boundary_sync).
+__device__ __forceinline__ void grid_barrier(unsigned* counter, unsigned target, bool run_ahead) {
     __threadfence();
-    asm volatile("fence.proxy.async;" ::: "memory");
-    __syncthreads();
+    if (!run_ahead) asm volatile("fence.proxy.async;" ::: "memory");
+    boundary_sync(run_ahead);
     if (threadIdx.x == 0) {
         atomicAdd(counter, 1u);
         while ((int)(*(volatile unsigned*)counter - target) < 0) {
         }
         __threadfence();
     }
-    __syncthreads();
+    boundary_sync(run_ahead);
 }
 
 }  // namespace tsk
