@@ -1542,7 +1542,7 @@ extern "C" int32_t b2k_basis_orthogonalize(b2k_ctx* ctx, b2k_vec v, const b2k_ve
             return b2k_fail(ctx, B2K_EINVAL, "basis_orthogonalize: v aliases basis vector %d", j);
     const bool f64 = ctx->dtype == B2K_F64;
     const bool fusable = fused_ok(ctx, k, pn.sharded, ctx->dtype);
-    const double eps = f64 ? 2.220446049250313e-16 : 1.1920929e-07;
+    const double eps = f64 ? 0x1p-52 : 0x1p-23;   // eps(T) of the IR loops (orthonormal.jl, lanczos.jl)
     const int NS_ = 2 * k + 4;   // slot of ||v||^2 results for unfused / MGS paths
 
     auto cgs_passes = [&](int passes) -> int32_t {   // leaves h in h_res[0..k), norm^2 in h_res[k]
@@ -1637,7 +1637,7 @@ extern "C" int32_t b2k_lanczos_expand(b2k_ctx* ctx, const b2k_op* op, const b2k_
         if (cols[j] == w) return b2k_fail(ctx, B2K_EINVAL, "lanczos_expand: w aliases the basis");
     const bool f64 = ctx->dtype == B2K_F64;
     const int K1 = k + 1;
-    const double eps = f64 ? 2.220446049250313e-16 : 1.1920929e-07;
+    const double eps = f64 ? 0x1p-52 : 0x1p-23;   // eps(T) of the IR loops (orthonormal.jl, lanczos.jl)
     // d_res slots
     const int S_H = 0;             // [0..K1) projection coefficients
     const int S_N = K1;            // ||w||^2

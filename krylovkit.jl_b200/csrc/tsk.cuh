@@ -25,6 +25,7 @@
 //   * reductions are deterministic: per-CTA partials at fixed slots, summed in CTA order
 //     by every consumer of the next phase (or by the finalize kernel).  No FP atomics.
 #pragma once
+#include <type_traits>
 #include "common.cuh"
 
 namespace tsk {
@@ -250,6 +251,12 @@ template <> struct VecOps<double> {
         acc = fma(q.x, x.x, acc);
         acc = fma(q.y, x.y, acc);
     }
+    // the elements of rows >= rt (r0 = row of q.x) become 0
+    __device__ static __forceinline__ double2 mask(double2 q, int r0, int rt) {
+        if (r0 >= rt) q.x = 0.0;
+        if (r0 + 1 >= rt) q.y = 0.0;
+        return q;
+    }
 };
 template <> struct VecOps<float> {
     __device__ static __forceinline__ void fma_acc(float& acc, const float4& q, const float4& x) {
@@ -257,6 +264,13 @@ template <> struct VecOps<float> {
         acc = fmaf(q.y, x.y, acc);
         acc = fmaf(q.z, x.z, acc);
         acc = fmaf(q.w, x.w, acc);
+    }
+    __device__ static __forceinline__ float4 mask(float4 q, int r0, int rt) {
+        if (r0 >= rt) q.x = 0.0f;
+        if (r0 + 1 >= rt) q.y = 0.0f;
+        if (r0 + 2 >= rt) q.z = 0.0f;
+        if (r0 + 3 >= rt) q.w = 0.0f;
+        return q;
     }
 };
 
@@ -398,28 +412,37 @@ __device__ __forceinline__ void consumer_phase(const PhaseParams<T>& p, const Sm
             for (int i = 0; i < NLD; ++i)
                 xr[i] = *reinterpret_cast<const V16*>(wb + VEC * lane + 32 * VEC * i);
             uint32_t ss = UPDATE ? s0 : st.s, pp = UPDATE ? ph0 : st.ph;
+            // The bulk copies of a ragged tile fill rows < rt only: the slot rows past them still hold an earlier
+            // tile's values (of whichever column used the slot then).  x is 0 there, but Inf * 0 is NaN, so the
+            // ragged tile zeroes those elements of q before the products; full tiles take the unmasked copy.
+            auto sweep = [&](auto masked) {
 #pragma unroll
-            for (int c = 0; c < MAXCH; ++c) {
-                if (c < nch) {
-                    if (!UPDATE) mbar_wait(sm.full + 8 * ss, pp);
-                    const T* slot = reinterpret_cast<const T*>(sm.raw + OFF_RING + ss * SLOT_BYTES);
+                for (int c = 0; c < MAXCH; ++c) {
+                    if (c < nch) {
+                        if (!UPDATE) mbar_wait(sm.full + 8 * ss, pp);
+                        const T* slot = reinterpret_cast<const T*>(sm.raw + OFF_RING + ss * SLOT_BYTES);
 #pragma unroll
-                    for (int cc = 0; cc < CPW; ++cc) {
-                        const int cj = cc * 8 + w;
-                        if (c * C + cj < p.k) {
-                            const T* colp = slot + cj * R;
+                        for (int cc = 0; cc < CPW; ++cc) {
+                            const int cj = cc * 8 + w;
+                            if (c * C + cj < p.k) {
+                                const T* colp = slot + cj * R;
 #pragma unroll
-                            for (int i = 0; i < NLD; ++i) {
-                                V16 q = *reinterpret_cast<const V16*>(colp + VEC * lane + 32 * VEC * i);
-                                VecOps<T>::fma_acc(acc_h[c][cc], q, xr[i]);
+                                for (int i = 0; i < NLD; ++i) {
+                                    V16 q = *reinterpret_cast<const V16*>(colp + VEC * lane + 32 * VEC * i);
+                                    if constexpr (decltype(masked)::value)
+                                        q = VecOps<T>::mask(q, VEC * lane + 32 * VEC * i, rt);
+                                    VecOps<T>::fma_acc(acc_h[c][cc], q, xr[i]);
+                                }
                             }
                         }
+                        __syncwarp();
+                        if (lane == 0) mbar_arrive(sm.empty + 8 * ss);
+                        if (++ss == NS) { ss = 0; pp ^= 1; }
                     }
-                    __syncwarp();
-                    if (lane == 0) mbar_arrive(sm.empty + 8 * ss);
-                    if (++ss == NS) { ss = 0; pp ^= 1; }
                 }
-            }
+            };
+            if (rt == R) sweep(std::false_type{});
+            else sweep(std::true_type{});
             if (!UPDATE) { st.s = ss; st.ph = pp; }
             buf ^= 1;
         }
