@@ -203,7 +203,7 @@ int32_t b2k_op_apply_adjoint(b2k_ctx* ctx, const b2k_op* op, b2k_vec x, b2k_vec 
 /* y = A x AND z = A'(A x) from ONE pass over a dense A (SURVEY §8f-4; the flagged one-pass mode of the
  * Golub-Kahan-Lanczos step: gkl.jl:308-323 reads A twice per step, `apply_adjoint` then `apply_normal`; with z
  * the host recovers A'u_{k+1} = (z - sum_j c_j A'u_j) / beta_k without the second pass).  x, z: length n_cols
- * (z must not alias x); y: length n_rows.  Dense operators with at most 1700 (Float32) / 850 (Float64) columns;
+ * (z must not alias x); y: length n_rows.  Dense operators with at most 1700 (Float32) / 846 (Float64) columns;
  * B2K_ENOTSUP otherwise.  Row-sharded contexts sum z over the ranks. */
 int32_t b2k_op_apply_normal_gram(b2k_ctx* ctx, const b2k_op* op, b2k_vec x, b2k_vec y, b2k_vec z);
 /* y = A x and dot = <v, y> in the same pass (lanczos.jl:297-298 `w = apply; α = inner(v,w)`) */

@@ -2196,7 +2196,7 @@ extern "C" int32_t b2k_pencil_rayleigh(b2k_ctx* ctx, const void* Pv, b2k_vec x, 
 // host recovers A'u_{k+1} = (z - sum_j c_j A'u_j) / beta_k from it (factorizations/gkl.py) without a second
 // pass.  The reduction over rows of y = A x is LOCAL to a row tile, so no grid-wide barrier is needed:
 //
-//   tile   = 32 rows x n columns of the column-major A (n <= 1700 Float32 / 850 Float64), parked in shared
+//   tile   = 32 rows x n columns of the column-major A (n <= 1700 Float32 / 846 Float64), parked in shared
 //            memory with a column stride of 33 words: conflict-free both for lane <-> row (the tile stores)
 //            and for lane <-> column (phase 2);
 //   load   : every thread issues 8 independent 16-byte loads (4 Float32 / 2 Float64 consecutive rows of one
@@ -2215,6 +2215,7 @@ namespace {
 #include "onepass_kernels.cuh"
 
 int g_onepass_variant = 0;       // 0: 32-row tiles, 3 CTAs per SM (A); 1: 64-row tiles, register-pipelined (B, Float32 n <= 512)
+int32_t g_onepass_launch[4] = {-1, 0, 0, 0};     // {variant, NZ, grid, ntiles} of the last launch (b2k_debug_onepass_launch)
 
 // per-CTA partials -> z (and the sum over the ranks of a row-sharded context)
 template <typename T>
@@ -2249,6 +2250,7 @@ int32_t onepass_w(b2k_ctx* ctx, b2k_op* op, const VecRef& x, const VecRef& y, co
     const int64_t ntiles = (op->ld + OPW_ROWS - 1) / OPW_ROWS;
     const int grid = (int)std::min<int64_t>(ntiles, (int64_t)ctx->num_sms);
     B2K_TRY(onepass_part(ctx, op, (size_t)grid * n * sizeof(double)));
+    g_onepass_launch[0] = 1; g_onepass_launch[1] = 0; g_onepass_launch[2] = grid; g_onepass_launch[3] = (int32_t)ntiles;
     const int pr = b2k_prof_begin(ctx, 8, 4.0 * ((double)op->n_rows * n + (double)op->n_rows + n));
     k_dense_onepass_w<<<grid, OPW_T, smem, ctx->stream>>>((const float*)op->A, op->ld, op->n_rows, n, (const float*)x.ptr,
                                                          (float*)y.ptr, op->part, ntiles);
@@ -2275,6 +2277,10 @@ int32_t onepass_t(b2k_ctx* ctx, b2k_op* op, const VecRef& x, const VecRef& y, co
     const int64_t ntiles = op->ld / OP_ROWS;
     const int grid = (int)std::min<int64_t>(ntiles, (int64_t)occ * ctx->num_sms);
     B2K_TRY(onepass_part(ctx, op, (size_t)grid * n * sizeof(double)));
+    g_onepass_launch[0] = 0;
+    g_onepass_launch[1] = n <= OP_T ? 1 : n <= 2 * OP_T ? 2 : n <= 4 * OP_T ? 4 : OP_ZMAX;
+    g_onepass_launch[2] = grid;
+    g_onepass_launch[3] = (int32_t)ntiles;
     const int pr = b2k_prof_begin(ctx, 8, (double)sizeof(T) * ((double)op->n_rows * n + (double)op->n_rows + n));
     kern<<<grid, OP_T, smem, ctx->stream>>>((const T*)op->A, op->ld, op->n_rows, n, (const T*)x.ptr,
                                                            (T*)y.ptr, op->part, ntiles);
@@ -2312,6 +2318,14 @@ extern "C" int32_t b2k_op_apply_normal_gram(b2k_ctx* ctx, const b2k_op* op, b2k_
 extern "C" int32_t b2k_debug_set_onepass_variant(int32_t v) {
     if (v < 0 || v > 1) return B2K_EINVAL;
     g_onepass_variant = v;
+    return B2K_OK;
+}
+
+// the last one-pass launch that passed its checks: {variant (0 = A, 1 = B, -1 = none yet), NZ (variant A's template
+// instance, 0 for B), grid, ntiles} — the grid depends on the occupancy, which a test of the summation order needs
+extern "C" int32_t b2k_debug_onepass_launch(int32_t* out) {
+    if (!out) return B2K_EINVAL;
+    for (int i = 0; i < 4; ++i) out[i] = g_onepass_launch[i];
     return B2K_OK;
 }
 

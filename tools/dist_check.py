@@ -55,6 +55,55 @@ def watchdog_check(rank, world, local):
     dist.destroy_process_group()
 
 
+def onepass_check(shard, n_global, rank, world, local, dev, use_nccl):
+    """b2k_op_apply_normal_gram on a row-sharded splitmix matrix (oracle/onepass_restate.py states the order), on a
+    context of its own per type: Float64 with 300 columns, Float32 with 1100 (two 1024-column pieces of the peer
+    all-reduce when NCCL is off; more than the 846 columns a Float64 tile may have).  Each rank's y is its own rows'
+    restatement with the grid that rank launched; z, on every rank, is the rank-ordered sum from 0.0 of the ranks'
+    restated Float64 sums, rounded to T.  With NCCL, more than 1024 columns go through ncclAllReduce, whose order is
+    NCCL's: with three or more ranks only the Float64 bound is asserted there (two addends give the same bits in
+    either order)."""
+    import ctypes
+    import shutil
+    import tempfile
+    from krylovkit_jl_b200.operators import apply_normal_gram
+    from oracle import onepass_restate as rs
+    tmp = tempfile.mkdtemp(prefix="onepass_fma_")
+    try:
+        fma = rs.load_fma(tmp)
+        lib = kk._lib.load()
+        for dt, ncols, seed in ((np.float64, 300, 41), (np.float32, 1100, 43)):
+            uid = sharding.broadcast_nccl_uid(dist, lib)
+            ctx = kk.B200Context(shard.n_local, 4, dtype=dt, device=local, rank=rank, nranks=world, nccl_uid=uid,
+                                 n_global=n_global, row_offset=shard.row_offset)
+            sv = ctx.add_space(ncols, 4, sharded=False)
+            op = kk.B200Dense.splitmix(ctx, shard.n_local, ncols, seed, sv)
+            A = ko.dense_splitmix(seed, shard.n_local, ncols, dtype=dt, row0=shard.row_offset, m_global=n_global)
+            x = (ko.splitmix_vector(seed + 1, ncols) - 0.5).astype(dt)
+            y, z = apply_normal_gram(op, ctx.from_host(x, space=sv))
+            info = (ctypes.c_int32 * 4)()
+            assert lib.b2k_debug_onepass_launch(info) == 0 and info[0] == 0, list(info)
+            ry, _, dres, _ = rs.apply_normal_gram(A, x, 0, info[2], fma)
+            u = np.uint64 if dt == np.float64 else np.uint32
+            assert np.array_equal(y.to_host().view(u), ry.view(u)), (rank, ncols)
+            parts = [torch.zeros(ncols, dtype=torch.float64, device=dev) for _ in range(world)]
+            dist.all_gather(parts, torch.from_numpy(dres).to(dev))
+            per_rank = [p.cpu().numpy() for p in parts]
+            want = rs.rank_sum(per_rank)
+            zh = z.to_host()
+            if use_nccl and ncols > 1024 and world > 2:
+                bound = world * 2.0 ** -53 * np.sum(np.abs(per_rank), axis=0) + np.abs(want) * np.finfo(dt).eps
+                assert np.all(np.abs(zh - want) <= bound), (rank, ncols)
+            else:
+                assert np.array_equal(zh.view(u), want.astype(dt).view(u)), (rank, ncols)
+            del y, z, op
+            ctx.close()
+    finally:
+        shutil.rmtree(tmp, ignore_errors=True)
+    if rank == 0:
+        print(f"dist_check: one-pass GKL step bit-equal to the restatement on {world} ranks")
+
+
 def main():
     rank, world, local = int(os.environ["RANK"]), int(os.environ["WORLD_SIZE"]), int(os.environ["LOCAL_RANK"])
     one_gpu = os.environ.get("B2K_ONE_GPU", "") == "1"
@@ -141,6 +190,7 @@ def main():
             print(f"dist_check ok on {world} ranks (short): Ritz values {res[1][0][:3]}")
         dist.barrier()
         ctx.close()
+        onepass_check(shard, n, rank, world, local, dev, use_nccl=not one_gpu)
         dist.destroy_process_group()
         return
     # 5. widened drivers (SURVEY §8f) on the sharded context: every scalar they see is all-reduced inside
@@ -188,6 +238,8 @@ def main():
         print(f"dist_check ok on {world} ranks: Ritz values {vals[:3]}")
     dist.barrier()
     ctx.close()
+    # the one-pass dense GKL step on the row shards: y and the per-rank sums against the restatement
+    onepass_check(shard, n, rank, world, local, dev, use_nccl=not one_gpu)
     dist.destroy_process_group()
 
 
