@@ -150,6 +150,9 @@ _PROTOS = {
     "b2k_debug_set_coop": (C.c_int32, [C.c_int32]),
     "b2k_debug_set_spmv_pipe": (C.c_int32, [C.c_int32]),
     "b2k_debug_set_spmv_variant": (C.c_int32, [C.c_int32]),
+    "b2k_debug_set_csr_compact": (C.c_int32, [C.c_int32]),
+    "b2k_debug_spmv_kernel": (C.c_int32, []),
+    "b2k_debug_csr_format": (C.c_int32, [c_op]),
     "b2k_debug_set_dmma": (C.c_int32, [C.c_int32]),
     "b2k_debug_set_transform": (C.c_int32, [C.c_int32]),
     "b2k_debug_transform_kernel": (C.c_int32, []),

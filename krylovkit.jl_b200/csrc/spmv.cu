@@ -41,6 +41,12 @@ struct b2k_op {
     int32_t* rowblk = nullptr;    // CTA row-block boundaries
     int32_t* pblk = nullptr;      // rowptr[rowblk[b]] (first nonzero of each block)
     int32_t  nblk = 0;
+    // compact copy of the CSR stream read by k_spmv_compact (build_compact; single-GPU CSR operators).  Each part is
+    // allocated only when it compressed losslessly; k_spmv_compact reads the plain array in place of a missing one.
+    // crp is null when neither values nor columns compressed: the operator then has no compact view.
+    float*    cvals = nullptr;    // Float64 contexts: every value as float (each one round-trips exactly)
+    int16_t*  ccol = nullptr;     // colidx - rowblk[tile] for every nonzero of every tile of <= SP_NNZ nonzeros
+    uint16_t* crp = nullptr;      // low 16 bits of rowptr
     double*  part = nullptr;      // per-CTA dot partials (CSR / stencil); per-CTA z partials of the one-pass dense step
     size_t   part_bytes = 0;      // size of `part` when the one-pass dense step allocated it
     // halo plan (dist)
@@ -425,6 +431,297 @@ k_spmv_pipe(const int32_t* __restrict__ rowptr, const int32_t* __restrict__ coli
             }
         }
     }
+}
+
+// ---------------------------------------------------------------------------------------
+// k_spmv_pipe on the compact copy of the matrix (finish_csr / build_compact, single-GPU operators):
+//   values   VS = float in a Float64 context when every value round-trips exactly ((double)(float)v bit-identical,
+//            no NaN), else T;
+//   columns  IS = int16 offsets col - rowblk[tile] when they fit for every nonzero of every tile of <= SP_NNZ
+//            nonzeros, else the int32 columns;
+//   rowptr   the low 16 bits of rowptr: inside a tile the offset rowptr[r] - pblk[tile] <= SP_NNZ is exact mod 2^16.
+// Each consumer rebuilds (T)value and the column and then does exactly what k_spmv_pipe does: the same products
+// (rounded in T), summed in the same CSR order by the same thread, the same dacc chain and CTA partials, so y, vout and
+// the dot are bit-identical to k_spmv_pipe at the same grid.  Long rows and tiles of more than SPP_RMAX rows read the
+// plain global arrays, as there.  With VS = float the products need T slots of their own: one buffer per CTA, so the
+// consumers meet once more per tile (before overwriting it) instead of growing every stage by SP_NNZ * 8 bytes.
+// The stages are half the size of k_spmv_pipe's, so the ring takes as many as fit beside 4 CTAs per SM.
+constexpr int SPC_TV = SP_NNZ + 16;          // staged entries of a 2- or 4-byte nonzero array (16-byte alignment slack)
+constexpr int SPC_CTAS = 4;
+constexpr int SPC_SMEM_MAX = 233472 / SPC_CTAS - 1024;     // 228 KB per SM, 1 KB reserved per CTA
+template <typename X> __device__ __forceinline__ int al_dn(int i) { return i & ~(16 / (int)sizeof(X) - 1); }
+template <typename X> __device__ __forceinline__ int al_up(int i) { return al_dn<X>(i + 16 / (int)sizeof(X) - 1); }
+template <typename T, typename VS, typename IS> struct SpcLayout {
+    static constexpr bool PROD = sizeof(VS) < sizeof(T);
+    static constexpr int VAL_BYTES = SPC_TV * (int)sizeof(VS);
+    static constexpr int COL_BYTES = SPC_TV * (int)sizeof(IS);
+    static constexpr int RP_BYTES = (SPP_RMAX + 16) * 2;
+    static constexpr int STAGE = VAL_BYTES + COL_BYTES + RP_BYTES;
+    static constexpr int PROD_BYTES = PROD ? SP_NNZ * (int)sizeof(T) : 0;
+    static constexpr int TAIL = 2 * 4 * 8 + 16 + 32 * 8 + 16;            // barriers of up to 4 stages, red, flag
+    static constexpr int NSTG = std::min(4, (SPC_SMEM_MAX - PROD_BYTES - TAIL) / STAGE);
+    static constexpr int OFF_PROD = NSTG * STAGE;
+    static constexpr int OFF_BAR = OFF_PROD + PROD_BYTES;
+    static constexpr int OFF_RED = OFF_BAR + 2 * NSTG * 8 + 16;
+    static constexpr int SMEM = OFF_RED + 32 * 8 + 16;
+    static_assert(NSTG >= 2 && SMEM <= SPC_SMEM_MAX, "compact SpMV stage ring does not fit 4 CTAs per SM");
+    static_assert(VAL_BYTES % 16 == 0 && COL_BYTES % 16 == 0 && RP_BYTES % 16 == 0, "TMA needs 16-byte offsets");
+};
+
+template <typename T, typename VS, typename IS>
+__global__ void __launch_bounds__(SPP_THREADS, SPC_CTAS)
+k_spmv_compact(const int32_t* __restrict__ rowptr, const int32_t* __restrict__ colidx, const T* __restrict__ vals,
+               const VS* __restrict__ cvals, const IS* __restrict__ ccol, const uint16_t* __restrict__ crp,
+               const T* __restrict__ x, T* __restrict__ y, const int32_t* __restrict__ rowblk,
+               const int32_t* __restrict__ pblk, int nblk, T a0, T a1, int shifted, const T* __restrict__ xs,
+               const T* __restrict__ dotv, double* __restrict__ part, unsigned* __restrict__ ticket,
+               double* __restrict__ out, const SpmvFuse fz) {
+    using LY = SpcLayout<T, VS, IS>;
+    constexpr int NSTG = LY::NSTG;
+    constexpr bool OFFS = sizeof(IS) == 2;     // columns staged as offsets from the tile's first row
+    extern __shared__ __align__(128) uint8_t smem[];
+    if (fz.stop && *reinterpret_cast<const volatile int*>(fz.stop)) return;
+    const uint32_t full = smem_u32(smem + LY::OFF_BAR), empty = full + NSTG * 8;
+    double* red = reinterpret_cast<double*>(smem + LY::OFF_RED);
+    int* flag = reinterpret_cast<int*>(smem + LY::OFF_RED + 32 * 8);
+    if (threadIdx.x == 0) {
+        for (int i = 0; i < NSTG; ++i) {
+            mbar_init(full + 8 * i, 1);
+            mbar_init(empty + 8 * i, SPP_CONS / 32);
+        }
+        fence_mbar_init();
+    }
+    __syncthreads();
+    const int lane = threadIdx.x & 31;
+    uint32_t s = 0, ph = 0;
+    if (threadIdx.x >= SPP_CONS) {
+        // ------------------------------ producer warp ------------------------------
+        int tile = blockIdx.x;
+        int d = 0;
+        if (tile < nblk && lane < 4) d = (lane < 2) ? rowblk[tile + lane] : pblk[tile + lane - 2];
+        for (; tile < nblk; tile += gridDim.x) {
+            const int r0 = __shfl_sync(0xffffffffu, d, 0), r1 = __shfl_sync(0xffffffffu, d, 1);
+            const int p0 = __shfl_sync(0xffffffffu, d, 2), p1 = __shfl_sync(0xffffffffu, d, 3);
+            const int nt = tile + gridDim.x;
+            if (nt < nblk && lane < 4) d = (lane < 2) ? rowblk[nt + lane] : pblk[nt + lane - 2];
+            mbar_wait(empty + 8 * s, ph ^ 1);
+            const int nnzb = p1 - p0, nrows = r1 - r0;
+            if (nnzb <= SP_NNZ) {
+                const int pv = al_dn<VS>(p0), pc = al_dn<IS>(p0), r0a = al_dn<uint16_t>(r0);
+                const uint32_t vb = (uint32_t)(al_up<VS>(p1) - pv) * (uint32_t)sizeof(VS);
+                const uint32_t cb = (uint32_t)(al_up<IS>(p1) - pc) * (uint32_t)sizeof(IS);
+                const uint32_t rb = nrows <= SPP_RMAX ? (uint32_t)(al_up<uint16_t>(r1 + 1) - r0a) * 2u : 0u;
+                const uint32_t st = smem_u32(smem + s * LY::STAGE);
+                if (lane == 0) mbar_expect_tx(full + 8 * s, vb + cb + rb);
+                __syncwarp();
+                if (fz.l2_hints) {
+                    const uint64_t pol = l2_policy_evict_first();
+                    if (lane == 0 && vb) bulk_g2s_hint(st, cvals + pv, vb, full + 8 * s, pol);
+                    if (lane == 1 && cb) bulk_g2s_hint(st + LY::VAL_BYTES, ccol + pc, cb, full + 8 * s, pol);
+                    if (lane == 2 && rb) bulk_g2s_hint(st + LY::VAL_BYTES + LY::COL_BYTES, crp + r0a, rb, full + 8 * s, pol);
+                } else {
+                    if (lane == 0 && vb) bulk_g2s(st, cvals + pv, vb, full + 8 * s);
+                    if (lane == 1 && cb) bulk_g2s(st + LY::VAL_BYTES, ccol + pc, cb, full + 8 * s);
+                    if (lane == 2 && rb) bulk_g2s(st + LY::VAL_BYTES + LY::COL_BYTES, crp + r0a, rb, full + 8 * s);
+                }
+            } else {
+                if (lane == 0) mbar_arrive(full + 8 * s);   // long row: consumers read global memory
+            }
+            if (++s == NSTG) { s = 0; ph ^= 1; }
+        }
+        return;
+    }
+    // ---------------------------------- consumers ----------------------------------
+    const int tid = threadIdx.x, w = tid >> 5;
+    const bool tr0 = fz.trace && blockIdx.x == 0 && tid == 0;
+    if (tr0) b2k_trace(fz.trace, 1);
+    if (tr0) b2k_trace(fz.trace, 2);
+    const bool scaled = fz.xscale != nullptr;
+    const T sc = scaled ? (T)(*fz.xscale) : (T)1;
+    T* const vout = reinterpret_cast<T*>(fz.vout);
+    const bool self = (vout != nullptr) || fz.dot_self;
+    const bool want_dot = (dotv != nullptr) || fz.dot_self;
+    const uint64_t pol_last = fz.l2_hints ? l2_policy_evict_last() : 0;
+    const T* const dsub = reinterpret_cast<const T*>(fz.dot_sub_vec);
+    const T dsc = dsub ? (T)(*fz.dot_sub_scale) : (T)0;
+    T dacc = (T)0;
+    // The x gather of the next tile is issued before the row sums of this one, so its latency (the first touch of an
+    // entry of x misses L2) overlaps them instead of stalling the CTA once per tile.
+    constexpr int U = SP_NNZ / SPP_CONS;
+    T xv[U];
+    auto gather = [&](uint32_t sg, int4 d) {
+        if (d.w - d.z > SP_NNZ) return;
+        const IS* cg = reinterpret_cast<const IS*>(smem + sg * LY::STAGE + LY::VAL_BYTES);
+        const int og = d.z - al_dn<IS>(d.z);
+#pragma unroll
+        for (int u = 0; u < U; ++u) {
+            const int i = tid + u * SPP_CONS;
+            if (i < d.w - d.z) xv[u] = __ldg(x + (OFFS ? d.x + (int)cg[og + i] : (int)cg[og + i]));
+        }
+    };
+    int tile = blockIdx.x;
+    int4 dn = make_int4(0, 0, 0, 0);
+    if (tile < nblk) {
+        dn = make_int4(rowblk[tile], rowblk[tile + 1], pblk[tile], pblk[tile + 1]);
+        mbar_wait(full, 0);
+        gather(0, dn);
+    }
+    for (; tile < nblk; tile += gridDim.x) {
+        const int r0 = dn.x, r1 = dn.y, p0 = dn.z, p1 = dn.w;
+        const int nt = tile + gridDim.x;
+        if (nt < nblk) dn = make_int4(rowblk[nt], rowblk[nt + 1], pblk[nt], pblk[nt + 1]);
+        const int nnzb = p1 - p0, nrows = r1 - r0;
+        const uint32_t s1 = s + 1 == NSTG ? 0 : s + 1, ph1 = s + 1 == NSTG ? ph ^ 1 : ph;
+        auto prefetch_next = [&]() {
+            if (nt < nblk) {
+                mbar_wait(full + 8 * s1, ph1);
+                gather(s1, dn);
+            }
+        };
+        if (nnzb <= SP_NNZ) {
+            uint8_t* const st = smem + s * LY::STAGE;
+            VS* vs = reinterpret_cast<VS*>(st);
+            const uint16_t* rs = reinterpret_cast<const uint16_t*>(st + LY::VAL_BYTES + LY::COL_BYTES);
+            const int offv = p0 - al_dn<VS>(p0), r0a = al_dn<uint16_t>(r0);
+            if (scaled) {
+#pragma unroll
+                for (int u = 0; u < U; ++u) xv[u] *= sc;      // v_j = r_j * (1/β), rounded like scale!!
+            }
+            T* pr;
+            if constexpr (LY::PROD) {
+                pr = reinterpret_cast<T*>(smem + LY::OFF_PROD);
+                named_bar_sync(1, SPP_CONS);                   // every row sum of the previous tile has read it
+            } else {
+                pr = reinterpret_cast<T*>(vs) + offv;          // in place, as k_spmv_pipe
+            }
+#pragma unroll
+            for (int u = 0; u < U; ++u) {
+                const int i = tid + u * SPP_CONS;
+                if (i < nnzb) pr[i] = (T)vs[offv + i] * xv[u];
+            }
+            named_bar_sync(1, SPP_CONS);
+            prefetch_next();
+            const bool rp_staged = nrows <= SPP_RMAX;
+            for (int r = r0 + tid; r < r1; r += SPP_CONS) {
+                T dv = (dotv && !fz.dot_self) ? __ldg(dotv + r) : (T)0;
+                const T xself = self ? __ldg(x + r) : (T)0;
+                const T xsr = shifted ? __ldg(xs + r) : (T)0;
+                const T dsv = dsub ? __ldg(dsub + r) : (T)0;
+                int a, b;
+                if (rp_staged) {
+                    a = (uint16_t)(rs[r - r0a] - (uint16_t)p0);
+                    b = (uint16_t)(rs[r + 1 - r0a] - (uint16_t)p0);
+                } else {
+                    a = rowptr[r] - p0;
+                    b = rowptr[r + 1] - p0;
+                }
+                T sum = (T)0;
+                for (int p = a; p < b; ++p) sum += pr[p];
+                if (shifted) sum = fma(a0, xsr, a1 * sum);
+                if (fz.l2_hints) st_hint(y + r, sum, pol_last);
+                else y[r] = sum;
+                if (self) {
+                    const T vn = xself * sc;
+                    if (vout) vout[r] = vn;
+                    if (fz.dot_self) dv = vn;
+                }
+                dacc = fma(dv, dsub ? fma(-dsc, dsv, sum) : sum, dacc);
+            }
+        } else {
+            double acc = 0.0;
+            for (int i = tid; i < nnzb; i += SPP_CONS) {
+                T xl = __ldg(x + colidx[p0 + i]);
+                if (scaled) xl *= sc;
+                acc += (double)mul_rn<T>(vals[p0 + i], xl);
+            }
+            acc = warp_sum(acc);
+            if (lane == 0) red[w] = acc;
+            named_bar_sync(1, SPP_CONS);
+            if (tid == 0) {
+                double tot = 0.0;
+                for (int i = 0; i < SPP_CONS / 32; ++i) tot += red[i];
+                T sum = (T)tot;
+                if (shifted) sum = fma(a0, xs[r0], a1 * sum);
+                y[r0] = sum;
+                T dv = (dotv && !fz.dot_self) ? dotv[r0] : (T)0;
+                if (self) {
+                    const T vn = __ldg(x + r0) * sc;
+                    if (vout) vout[r0] = vn;
+                    if (fz.dot_self) dv = vn;
+                }
+                if (want_dot) dacc = fma(dv, dsub ? fma(-dsc, dsub[r0], sum) : sum, dacc);
+            }
+            named_bar_sync(1, SPP_CONS);
+            prefetch_next();
+        }
+        fence_proxy_async();   // generic-proxy writes to the stage precede its reuse by the TMA unit
+        __syncwarp();
+        if (lane == 0) mbar_arrive(empty + 8 * s);
+        s = s1;
+        ph = ph1;
+    }
+    if (tr0) b2k_trace(fz.trace, 3);
+    if (want_dot) {
+        double v = warp_sum((double)dacc);
+        if (lane == 0) red[w] = v;
+        named_bar_sync(1, SPP_CONS);
+        if (tid == 0) {
+            double tot = 0.0;
+            for (int i = 0; i < SPP_CONS / 32; ++i) tot += red[i];
+            part[blockIdx.x] = tot;
+            __threadfence();
+            const unsigned t = atomicInc(ticket, gridDim.x - 1);
+            *flag = (t == gridDim.x - 1);
+        }
+        named_bar_sync(1, SPP_CONS);
+        if (*flag) {
+            __threadfence();
+            double v2 = 0.0;
+            const volatile double* pv = part;
+            for (int g = tid; g < (int)gridDim.x; g += SPP_CONS) v2 += pv[g];
+            v2 = warp_sum(v2);
+            named_bar_sync(1, SPP_CONS);
+            if (lane == 0) red[w] = v2;
+            named_bar_sync(1, SPP_CONS);
+            if (tid == 0) {
+                double tot = 0.0;
+                for (int i = 0; i < SPP_CONS / 32; ++i) tot += red[i];
+                *out = tot;
+                if (fz.trace) b2k_trace(fz.trace, 4);
+            }
+        }
+    }
+}
+
+// One CTA per tile: the compact copy of the tile's nonzeros and row pointers (k_spmv_compact), speculatively, and
+// bad |= 1 if a value does not round-trip through float (Float64 only), |= 2 if a column offset does not fit int16.
+template <typename T>
+__global__ void k_csr_compact(const int32_t* __restrict__ rowptr, const int32_t* __restrict__ colidx,
+                              const T* __restrict__ vals, const int32_t* __restrict__ rowblk,
+                              const int32_t* __restrict__ pblk, int nblk, float* __restrict__ cvals,
+                              int16_t* __restrict__ ccol, uint16_t* __restrict__ crp, int* __restrict__ bad) {
+    const int t = blockIdx.x;
+    const int r0 = rowblk[t], r1 = rowblk[t + 1], p0 = pblk[t], p1 = pblk[t + 1];
+    const bool normal = p1 - p0 <= SP_NNZ;
+    bool vbad = false, cbad = false;
+    for (int p = p0 + threadIdx.x; p < p1; p += blockDim.x) {
+        if (cvals) {
+            const double v = (double)vals[p];
+            const float f = (float)v;
+            vbad |= isnan(v) || __double_as_longlong((double)f) != __double_as_longlong(v);
+            cvals[p] = f;
+        }
+        if (normal) {
+            const int o = colidx[p] - r0;
+            cbad |= o < -32768 || o > 32767;
+            ccol[p] = (int16_t)o;
+        }
+    }
+    const int rend = r1 + (t == nblk - 1);
+    for (int r = r0 + threadIdx.x; r < rend; r += blockDim.x) crp[r] = (uint16_t)rowptr[r];
+    vbad = __syncthreads_or(vbad);
+    cbad = __syncthreads_or(cbad);
+    if (threadIdx.x == 0 && (vbad || cbad)) atomicOr(bad, (vbad ? 1 : 0) | (cbad ? 2 : 0));
 }
 
 // ---------------------------------------------------------------------------------------
@@ -1113,6 +1410,40 @@ __global__ void k_rowblocks(const int32_t* __restrict__ rowptr, int64_t n, int T
     rowblk[b] = (int32_t)lo;
 }
 
+// The compact copy of a CSR operator (k_spmv_compact): one pass writes every part and finds which ones are lossless,
+// then the parts that are not are freed.  Allocations are padded for the TMA segments, which round the end of a
+// tile up to 16 bytes.
+int32_t build_compact(b2k_ctx* ctx, b2k_op* op) {
+    const bool f64 = ctx->dtype == B2K_F64;
+    int* d_bad;
+    int h_bad = 0;
+    B2K_CUDA(ctx, B2K_DMALLOC(&d_bad, sizeof(int)));
+    B2K_CUDA(ctx, cudaMemsetAsync(d_bad, 0, sizeof(int), ctx->stream));
+    B2K_CUDA(ctx, B2K_DMALLOC(&op->crp, sizeof(uint16_t) * (op->n_rows + 1 + 16)));
+    B2K_CUDA(ctx, B2K_DMALLOC(&op->ccol, sizeof(int16_t) * (op->nnz + 16)));
+    if (f64) B2K_CUDA(ctx, B2K_DMALLOC(&op->cvals, sizeof(float) * (op->nnz + 16)));
+    if (f64)
+        k_csr_compact<double><<<op->nblk, 256, 0, ctx->stream>>>(op->rowptr, op->colidx, (const double*)op->vals,
+                                                                 op->rowblk, op->pblk, op->nblk, op->cvals, op->ccol,
+                                                                 op->crp, d_bad);
+    else
+        k_csr_compact<float><<<op->nblk, 256, 0, ctx->stream>>>(op->rowptr, op->colidx, (const float*)op->vals,
+                                                                op->rowblk, op->pblk, op->nblk, nullptr, op->ccol,
+                                                                op->crp, d_bad);
+    B2K_LAUNCH_CHECK(ctx);
+    B2K_CUDA(ctx, cudaMemcpyAsync(&h_bad, d_bad, sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
+    B2K_TRY(b2k_stream_sync(ctx));
+    B2K_DFREE(d_bad);
+    auto drop = [&](auto*& p) {
+        B2K_DFREE(p);
+        p = nullptr;
+    };
+    if (op->cvals && (h_bad & 1)) drop(op->cvals);
+    if (h_bad & 2) drop(op->ccol);
+    if (!op->cvals && !op->ccol) drop(op->crp);
+    return B2K_OK;
+}
+
 int32_t finish_csr(b2k_ctx* ctx, b2k_op* op) {
     const int64_t n = op->n_rows;
     int* d_stats;
@@ -1152,6 +1483,8 @@ int32_t finish_csr(b2k_ctx* ctx, b2k_op* op) {
     k_pblk<<<(op->nblk + 1 + 255) / 256, 256, 0, ctx->stream>>>(op->rowptr, op->rowblk, op->nblk + 1, op->pblk);
     B2K_LAUNCH_CHECK(ctx);
     B2K_CUDA(ctx, B2K_DMALLOC(&op->part, sizeof(double) * std::max(1, op->nblk)));
+    // row-sharded operators keep the plain arrays: their halo columns (n_loc + j) do not fit 16-bit offsets
+    if (ctx->nranks == 1 && op->nnz > 0) return build_compact(ctx, op);
     return B2K_OK;
 }
 
@@ -1585,7 +1918,8 @@ extern "C" int32_t b2k_op_create_dense_splitmix(b2k_ctx* ctx, b2k_op** out, int6
 
 void b2k_op_release(b2k_ctx* ctx, b2k_op* op) {
     cudaStream_t st = ctx ? ctx->stream : nullptr;
-    void* ptrs[] = {op->rowptr, op->colidx, op->vals, op->rowblk, op->pblk, op->part, op->halo, op->xall, op->A};
+    void* ptrs[] = {op->rowptr, op->colidx, op->vals, op->rowblk, op->pblk, op->part, op->halo, op->xall, op->A,
+                    op->cvals, op->ccol, op->crp};
     for (void* p : ptrs) b2k_dfree(p, st);     // stream-ordered: pending kernels finish first
     delete op;
 }
@@ -1782,6 +2116,26 @@ extern "C" int32_t b2k_debug_set_spmv_variant(int32_t v) {
     return B2K_OK;
 }
 
+// k_spmv_compact in place of k_spmv_pipe for operators with a compact view: on unless B2K_CSR_COMPACT=0
+static bool g_csr_compact = true;
+// the CSR SpMV kernel the last apply launched (b2k_debug_spmv_kernel): 0 = none yet, 1 = k_spmv_stream,
+// 2 = k_spmv_pipe, 3 = k_spmv_compact
+static int g_spmv_kernel = 0;
+
+extern "C" int32_t b2k_debug_set_csr_compact(int32_t on) {
+    g_csr_compact = on != 0;
+    return B2K_OK;
+}
+
+extern "C" int32_t b2k_debug_spmv_kernel(void) { return g_spmv_kernel; }
+
+// the compact view of an operator: 0 = none, else 4 (16-bit row pointers) | 2 (16-bit column offsets) | 1 (Float32
+// values in a Float64 context)
+extern "C" int32_t b2k_debug_csr_format(const b2k_op* op) {
+    if (!op || !op->crp) return 0;
+    return 4 | (op->ccol ? 2 : 0) | (op->cvals ? 1 : 0);
+}
+
 // opt in to > 48 KB dynamic shared memory for the pipelined SpMV (called per context)
 int32_t b2k_spmv_init(b2k_ctx* ctx) {
     B2K_CUDA(ctx, cudaFuncSetAttribute(k_spmm_pipe<double>, cudaFuncAttributeMaxDynamicSharedMemorySize,
@@ -1796,6 +2150,15 @@ int32_t b2k_spmv_init(b2k_ctx* ctx) {
                                        SppLayout<double, 2>::SMEM));
     B2K_CUDA(ctx, cudaFuncSetAttribute((k_spmv_pipe<float, 2, 4>), cudaFuncAttributeMaxDynamicSharedMemorySize,
                                        SppLayout<float, 2>::SMEM));
+#define SPC_ATTR(T, VS, IS)                                                                                    \
+    B2K_CUDA(ctx, cudaFuncSetAttribute((k_spmv_compact<T, VS, IS>), cudaFuncAttributeMaxDynamicSharedMemorySize, \
+                                       SpcLayout<T, VS, IS>::SMEM))
+    SPC_ATTR(double, float, int16_t);
+    SPC_ATTR(double, float, int32_t);
+    SPC_ATTR(double, double, int16_t);
+    SPC_ATTR(float, float, int16_t);
+#undef SPC_ATTR
+    if (const char* e = getenv("B2K_CSR_COMPACT")) g_csr_compact = e[0] != '0';
 #define PEN_ATTR(T, MODE)                                                                                      \
     B2K_CUDA(ctx, cudaFuncSetAttribute((k_spmv_pencil<T, PEN_NSTG, PenCtas<T>::N, MODE>),                     \
                                        cudaFuncAttributeMaxDynamicSharedMemorySize, PenLayout<T, PEN_NSTG>::SMEM))
@@ -1939,10 +2302,31 @@ int32_t b2k_enqueue_apply_fused(b2k_ctx* ctx, const b2k_op* op, const VecRef& x,
         B2K_LAUNCH_CHECK(ctx);
         return B2K_OK;
     }
-    // algorithmic bytes: matrix + x + y, plus the normalised copy of x a chained Lanczos step stores (fz.vout)
-    const int pr = b2k_prof_begin(ctx, 0, (double)op->nnz * (ctx->esize + 4) + 4.0 * (op->n_rows + 1) +
+    // algorithmic bytes: matrix (as streamed) + x + y, plus the normalised copy of x a chained Lanczos step stores
+    // (fz.vout)
+    const bool compact = g_spmv_pipe && g_csr_compact && op->crp != nullptr;
+    const double vbytes = (compact && op->cvals) ? 4.0 : (double)ctx->esize, cbytes = (compact && op->ccol) ? 2.0 : 4.0;
+    const int pr = b2k_prof_begin(ctx, 0, (double)op->nnz * (vbytes + cbytes) + (compact ? 2.0 : 4.0) * (op->n_rows + 1) +
                                               (fz.vout ? 3.0 : 2.0) * ctx->esize * op->n_rows);
-    if (g_spmv_pipe) {
+    g_spmv_kernel = compact ? 3 : (g_spmv_pipe ? 2 : 1);
+    if (compact) {
+        // the grid of k_spmv_pipe's variant: the CTA partials of the dot, and so its rounding, stay the same
+        const int per_sm = g_spmv_variant == 1 ? 4 : 3;
+        const int grid = std::min(op->nblk, per_sm * ctx->num_sms);
+#define LAUNCH_C(T, VS, IS, cv, cc)                                                                            \
+    k_spmv_compact<T, VS, IS><<<grid, SPP_THREADS, SpcLayout<T, VS, IS>::SMEM, ctx->stream>>>(                 \
+        op->rowptr, op->colidx, (const T*)op->vals, (const VS*)(cv), (const IS*)(cc), op->crp, (const T*)xsrc, \
+        (T*)y.ptr, op->rowblk, op->pblk, op->nblk, (T)a0, (T)a1, shifted ? 1 : 0, (const T*)x.ptr,            \
+        dotv ? (const T*)dotv->ptr : nullptr, op->part, ctx->d_sync, out, fz)
+        if (ctx->dtype == B2K_F64) {
+            if (op->cvals && op->ccol) LAUNCH_C(double, float, int16_t, op->cvals, op->ccol);
+            else if (op->cvals) LAUNCH_C(double, float, int32_t, op->cvals, op->colidx);
+            else LAUNCH_C(double, double, int16_t, op->vals, op->ccol);
+        } else {
+            LAUNCH_C(float, float, int16_t, op->vals, op->ccol);
+        }
+#undef LAUNCH_C
+    } else if (g_spmv_pipe) {
         const int per_sm = g_spmv_variant == 1 ? 4 : 3;
         const int grid = std::min(op->nblk, per_sm * ctx->num_sms);
 #define LAUNCH_V(T, NS, MB)                                                                    \
