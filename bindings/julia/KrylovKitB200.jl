@@ -521,6 +521,27 @@ function bicgstab_chain!(A::B200CSR, x::B200Vec, r::B200Vec, rs::B200Vec, p::B20
                          Float64(α₁), Float64(ρ), Float64(ρold), Float64(α), Float64(ω), Float64(tol), Int32(nsteps), rec, done))
     return rec[:, 1:done[]]
 end
+# minres_chain!: up to `nsteps` MINRES iterations (Paige & Saunders: Lanczos + Givens QR) for (α₀ + α₁ A) x = b with one
+# host synchronisation; two launches per iteration (the SpMV normalises p_cur by 1/β_k while gathering and returns
+# α = <v_k, q>; one streaming pass updates p, d and x and runs the scalar recurrence).  `state` is the 8-vector
+# (β_k, 1/β_k, 1/β_{k-1}, c, s, δ̄, ε, φ̄) — (‖r‖, 1/‖r‖, 0, -1, 0, 0, 0, ‖r‖) for a process started from the residual r
+# in p_cur with p_prev = d1 = d2 = 0 — and is advanced in place.  Returns an 8 × done matrix, one column per iteration:
+# (α, β_{k+1}, γ, φ, |φ̄|, stop code, δ, ε); stop code 1: |φ̄| < tol, 2: γ == 0, 3: β_{k+1} == 0.  When `done` is odd
+# p_prev / p_cur and d1 / d2 have swapped roles: the caller swaps its names (linsolve below does).
+function minres_chain!(A::B200CSR, x::B200Vec, p_prev::B200Vec, p_cur::B200Vec, q::B200Vec, d1::B200Vec, d2::B200Vec,
+                       α₀::Real, α₁::Real, state::Vector{Float64}, tol::Real, nsteps::Integer)
+    rec, done, out = zeros(Float64, 8, nsteps), Ref{Int32}(0), zeros(Float64, 8)
+    check(x.ctx.h, ccall((:b2k_minres_chain, lib), Cint,
+                         (Ptr{Cvoid}, Ptr{Cvoid}, Int32, Int32, Int32, Int32, Int32, Int32, Float64, Float64, Ptr{Float64},
+                          Float64, Int32, Ptr{Float64}, Ptr{Float64}, Ref{Int32}),
+                         x.ctx.h, A.h, x.handle, p_prev.handle, p_cur.handle, q.handle, d1.handle, d2.handle, Float64(α₀),
+                         Float64(α₁), state, Float64(tol), Int32(nsteps), rec, out, done))
+    copyto!(state, out)
+    return rec[:, 1:done[]]
+end
+# KrylovKit.linsolve(A::B200CSR, b, x₀, alg::MINRES, a₀, a₁): KrylovKit declares `MINRES` and has no method for it; the
+# driver is krylovkit.jl_b200/linsolve.py::_minres, statement for statement — initial residual, batches of
+# minres_chain!, the explicit residual behind every |φ̄| < tol, restart from x when it disagrees.
 # KrylovKit.linsolve(A::B200CSR, b, x₀, alg::CG / BiCGStab, a₀, a₁) are the reference drivers (cg.jl, bicgstab.jl)
 # with their loop bodies replaced by the calls above — krylovkit.jl_b200/linsolve.py::_cg/_bicgstab is that code,
 # statement for statement, and is what the test-suite runs.

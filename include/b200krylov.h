@@ -275,6 +275,31 @@ int32_t b2k_bicgstab_chain(b2k_ctx* ctx, const b2k_op* op, b2k_vec x, b2k_vec r,
                            double alpha, double omega, double tol, int32_t nsteps, double* rec_out,
                            int32_t* steps_done);
 
+/* Up to `nsteps` MINRES iterations (Paige & Saunders 1975: Lanczos + Givens QR, unpreconditioned) for the symmetric
+ * system (a0 + a1*A) x = b, enqueued back to back with ONE host synchronisation per call.  Two launches per iteration k:
+ *   q <- (a0 + a1*A) v_k with v_k = p_cur/beta_k formed while gathering (p_cur stays unnormalised) and
+ *        alpha = <v_k, q> in the epilogue;
+ *   one streaming pass (9 vector sweeps): p_{k} = q - alpha v_k - beta_k v_{k-1} over p_prev, beta_{k+1} = ||p_k||, and
+ *        the direction / solution update of iteration k-1, d = (v_{k-1} - delta d1 - eps d2)/gamma over d2,
+ *        x += phi d (it needs gamma_{k-1}, hence beta_k: one iteration late); the scalar recurrence (delta, gamma,
+ *        c, s, phi, phibar) follows in the same kernel, in Float64.
+ * A last launch applies the update still pending, so on return x is the iterate of the last recorded iteration.
+ * After the call the roles have rotated *steps_done times: if *steps_done is odd, p_prev / p_cur have swapped and
+ * so have d1 / d2 (p_cur is again the latest Lanczos vector, d1 the latest direction).
+ * state_in / state_out, 8 doubles: {beta_k, 1/beta_k, 1/beta_{k-1}, c, s, deltabar, eps, phibar}; a process
+ * started from the residual r (p_cur = r, p_prev = d1 = d2 = 0) has {||r||, 1/||r||, 0, -1, 0, 0, 0, ||r||}.
+ * Handing state_out to the next call continues the same process bit for bit.
+ * rec_out: 8 doubles per completed iteration {alpha, beta_{k+1}, gamma, phi, |phibar|, stop code, delta, eps};
+ * stop code 1 = |phibar| < tol, 2 = gamma == 0 (singular on the Krylov space; that iteration leaves x unchanged and
+ * sets d to zero), 3 = beta_{k+1} == 0; the stopping iteration is the last of *steps_done and the launches behind
+ * it do nothing.  Vectors are rounded exactly as the scale!! / add!! sequence they replace; alpha and beta are
+ * deterministic per-CTA sums (as b2k_op_apply_dot).  nsteps is capped at 511.
+ * Single GPU, CSR and stencil operators: B2K_ENOTSUP for dense operators and row-sharded contexts; B2K_EDIM when a
+ * length differs; B2K_EINVAL when two vectors are the same.  A refused call writes nothing. */
+int32_t b2k_minres_chain(b2k_ctx* ctx, const b2k_op* op, b2k_vec x, b2k_vec p_prev, b2k_vec p_cur, b2k_vec q,
+                         b2k_vec d1, b2k_vec d2, double a0, double a1, const double* state_in, double tol,
+                         int32_t nsteps, double* rec_out, double* state_out, int32_t* steps_done);
+
 /* ---------------------------------------------- basis (OrthonormalBasis) ---- */
 /* project!!(y, b, x, alpha, beta, r): h[j] = beta*h[j] + alpha*<b[cols[j]], x>
  * — src/orthonormal.jl:88-118.  h is a HOST vector (orthonormal.jl:374, arnoldi.jl:212). */

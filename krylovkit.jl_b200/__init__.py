@@ -12,7 +12,7 @@ from . import _lib
 from ._lib import B200Error, DimensionMismatch, LibraryMissing
 from .algorithms import (Arnoldi, BiArnoldi, BiCGStab, BlockLanczos, CG, ClassicalGramSchmidt, ClassicalGramSchmidt2,
                          ClassicalGramSchmidtIR, ConvergenceInfo, GKL, GMRES, GolubYe, KrylovDefaults,
-                         Lanczos, LSMR, ModifiedGramSchmidt, ModifiedGramSchmidt2,
+                         Lanczos, LSMR, MINRES, ModifiedGramSchmidt, ModifiedGramSchmidt2,
                          ModifiedGramSchmidt2Blocked, ModifiedGramSchmidtIR, Orthogonalizer, cgs, cgs2, cgsr, mgs,
                          mgs2, mgs2b, mgsr)
 from .operators import (B200CSR, B200Dense, B200Operator, B200Pencil, apply, apply_adjoint, apply_normal,

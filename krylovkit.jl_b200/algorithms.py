@@ -175,6 +175,15 @@ class CG:
 
 
 @dataclass(frozen=True)
+class MINRES:
+    """src/algorithms.jl:397-427 (declared there, without a driver): MINRES for real symmetric systems that need
+    not be positive definite.  linsolve.py::_minres fixes the recurrence (Paige & Saunders 1975)."""
+    maxiter: int = KrylovDefaults.maxiter
+    tol: float = KrylovDefaults.tol
+    verbosity: int = KrylovDefaults.verbosity
+
+
+@dataclass(frozen=True)
 class BiCGStab:
     """src/algorithms.jl:457-481."""
     maxiter: int = KrylovDefaults.maxiter

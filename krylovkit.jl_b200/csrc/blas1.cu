@@ -620,6 +620,145 @@ k_bicg_xr(T* __restrict__ x, T* __restrict__ r, const T* __restrict__ rs, const 
     }
 }
 
+// ---- MINRES (Paige & Saunders 1975, Lanczos + Givens QR; b2k_minres_chain) ----
+// Scalar state of the recurrence, on the device for the length of a call.  At the start of iteration k:
+// p_cur = p_{k-1} (unnormalised, v_k = p_cur * INVB), p_prev = p_{k-2} (v_{k-1} = p_prev * INVB_PREV).
+// P* = the direction / solution update of iteration k-1, which needs gamma_{k-1} and so beta_k: it is applied by the
+// kernel of iteration k (or by the flush launch); PEND says there is one.  DONE counts the iterations this call has
+// run: it fixes which buffer plays which role (the roles rotate with every iteration, skipped launches do not count).
+enum { MR_BETA = 0, MR_INVB, MR_INVB_PREV, MR_C, MR_S, MR_DBAR, MR_EPS, MR_PHIBAR,
+       MR_PDELTA, MR_PEPS, MR_PINVG, MR_PPHI, MR_PEND, MR_DONE, MR_NSTATE = 16 };
+
+struct MinresChain {
+    double* st;
+    double* rec;            // {alpha, beta_{k+1}, gamma, phi, |phibar|, stop code, delta, eps_k}
+    int* stop;
+    const double* alpha;    // <v_k, q> from the SpMV epilogue
+    double tol;
+};
+
+// One pass per MINRES iteration k (LANCZOS), after q = (a0 + a1 A) v_k:
+//   p_k = (q - alpha v_k) - beta_k v_{k-1}, sum p_k^2              [two add!! of the literal driver]
+//   d_{k-1} = ((v_{k-1} - delta d_{k-2}) - eps d_{k-3}) / gamma    [two add!!, one scale!!]
+//   x += phi d_{k-1}                                               [one add!!]
+// v_{k-1} = rn(p_prev * 1/beta_{k-1}) and v_k are formed in registers exactly as scale!! rounds them; p_k goes over
+// p_{k-2}, d_{k-1} over d_{k-3}.  Reads q, p_cur, p_prev, d1, d2, x and writes p, d, x: 9 W.  The last CTA then runs the
+// scalar recurrence of iteration k in Float64, every product and sum rounded on its own (no fma contraction), so a
+// host restatement in plain double arithmetic gives the same bits.
+// !LANCZOS is the flush launch: only the pending direction / solution update, whether or not the chain has stopped.
+template <typename T, bool LANCZOS>
+__global__ void __launch_bounds__(BT)
+k_minres_step(T* __restrict__ x, T* pA, T* pB, const T* __restrict__ q, T* dA, T* dB, int64_t n,
+              double* __restrict__ part, unsigned* __restrict__ ticket, const MinresChain ch) {
+    __shared__ double red[32];
+    __shared__ bool last;
+    if (LANCZOS && *reinterpret_cast<const volatile int*>(ch.stop)) return;
+    const volatile double* st = ch.st;
+    const bool pend = st[MR_PEND] != 0.0;
+    if (!LANCZOS && !pend) return;
+    const int done = (int)st[MR_DONE];
+    T* const pp = (done & 1) ? pB : pA;
+    const T* const pc = (done & 1) ? pA : pB;
+    const bool dswap = done > 0 && ((done - 1) & 1);        // direction updates applied so far: done - 1
+    const T* const d1 = dswap ? dB : dA;
+    T* const d2 = dswap ? dA : dB;
+    const double alpha = LANCZOS ? *ch.alpha : 0.0, beta = st[MR_BETA], invb = st[MR_INVB];
+    const T ip = (T)st[MR_INVB_PREV], ic = (T)invb, na = (T)(-alpha), nb = (T)(-beta);
+    const T nd = (T)(-st[MR_PDELTA]), ne = (T)(-st[MR_PEPS]), ig = (T)st[MR_PINVG], ph = (T)st[MR_PPHI];
+    constexpr int V = Vec16<T>::N;
+    const int64_t nv = n / V;
+    const int64_t stride = (int64_t)gridDim.x * BT;
+    T acc = 0;
+    auto each = [&](T pv, T cv, T qv, T av, T bv, T& xv, T& pout, T& dout) {
+        const T vp = mul_rn(pv, ip);
+        if (LANCZOS) {
+            pout = fma(nb, vp, fma(na, mul_rn(cv, ic), qv));
+            acc = fma(pout, pout, acc);
+        }
+        if (pend) {
+            dout = mul_rn(fma(ne, bv, fma(nd, av, vp)), ig);
+            xv = fma(ph, dout, xv);
+        }
+    };
+    B2K_TRIP(2) {
+        T pv[2][V], cv[2][V] = {}, qv[2][V] = {}, av[2][V] = {}, bv[2][V] = {}, xv[2][V] = {};
+        B2K_EACH(2, u, i) {
+            vload<T>(pp + i * V, pv[u]);
+            if (LANCZOS) {
+                vload<T>(pc + i * V, cv[u]);
+                vload<T>(q + i * V, qv[u]);
+            }
+            if (pend) {
+                vload<T>(d1 + i * V, av[u]);
+                vload<T>(d2 + i * V, bv[u]);
+                vload<T>(x + i * V, xv[u]);
+            }
+        }
+        B2K_EACH(2, u, i) {
+#pragma unroll
+            for (int j = 0; j < V; ++j) each(pv[u][j], cv[u][j], qv[u][j], av[u][j], bv[u][j], xv[u][j], pv[u][j], bv[u][j]);
+            if (LANCZOS) vstore<T>(pp + i * V, pv[u]);
+            if (pend) {
+                vstore<T>(d2 + i * V, bv[u]);
+                vstore<T>(x + i * V, xv[u]);
+            }
+        }
+    }
+    if (blockIdx.x == 0 && threadIdx.x < (n - nv * V)) {
+        const int64_t i = nv * V + threadIdx.x;
+        T xv = pend ? x[i] : (T)0, pout = 0, dout = 0;
+        each(pp[i], LANCZOS ? pc[i] : (T)0, LANCZOS ? q[i] : (T)0, pend ? d1[i] : (T)0, pend ? d2[i] : (T)0, xv, pout, dout);
+        if (LANCZOS) pp[i] = pout;
+        if (pend) {
+            d2[i] = dout;
+            x[i] = xv;
+        }
+    }
+    if (!LANCZOS) return;
+    const double sblk = block_sum((double)acc, red);
+    if (threadIdx.x == 0) {
+        part[blockIdx.x] = sblk;
+        __threadfence();
+        const unsigned t = atomicInc(ticket, gridDim.x - 1);
+        last = (t == gridDim.x - 1);
+    }
+    __syncthreads();
+    if (!last) return;
+    __threadfence();
+    double v = 0.0;
+    const volatile double* pv2 = part;
+    for (int g = threadIdx.x; g < (int)gridDim.x; g += BT) v += pv2[g];
+    const double tot = block_sum(v, red);
+    if (threadIdx.x != 0) return;
+    const double bn = sqrt(tot);                                        // beta_{k+1}
+    const double c0 = st[MR_C], s0 = st[MR_S], dbar = st[MR_DBAR], eps = st[MR_EPS], phibar = st[MR_PHIBAR];
+    const double delta = __dadd_rn(__dmul_rn(c0, dbar), __dmul_rn(s0, alpha));
+    const double gbar = __dadd_rn(__dmul_rn(s0, dbar), -__dmul_rn(c0, alpha));
+    const double gamma = sqrt(__dadd_rn(__dmul_rn(gbar, gbar), __dmul_rn(bn, bn)));
+    // gamma == 0: the shifted operator is singular on the Krylov space.  The pending update is kept, with zero
+    // weights (d_k = 0, x unchanged), so the roles rotate the same way on every exit.
+    const bool sing = gamma == 0.0;
+    const double c = sing ? 0.0 : __ddiv_rn(gbar, gamma), s = sing ? 0.0 : __ddiv_rn(bn, gamma);
+    const double phi = sing ? 0.0 : __dmul_rn(c, phibar), phibar_n = sing ? phibar : __dmul_rn(s, phibar);
+    const double code = sing ? 2.0 : (fabs(phibar_n) < ch.tol ? 1.0 : (bn == 0.0 ? 3.0 : 0.0));
+    double* w = ch.st;
+    w[MR_INVB_PREV] = invb;
+    w[MR_BETA] = bn;
+    w[MR_INVB] = __ddiv_rn(1.0, bn);
+    w[MR_C] = c; w[MR_S] = s;
+    w[MR_DBAR] = -__dmul_rn(c0, bn);
+    w[MR_EPS] = __dmul_rn(s0, bn);
+    w[MR_PHIBAR] = phibar_n;
+    w[MR_PDELTA] = delta; w[MR_PEPS] = eps;
+    w[MR_PINVG] = sing ? 0.0 : __ddiv_rn(1.0, gamma);
+    w[MR_PPHI] = phi;
+    w[MR_PEND] = 1.0;
+    w[MR_DONE] = (double)(done + 1);
+    ch.rec[0] = alpha; ch.rec[1] = bn; ch.rec[2] = gamma; ch.rec[3] = phi; ch.rec[4] = fabs(phibar_n);
+    ch.rec[5] = code; ch.rec[6] = delta; ch.rec[7] = eps;
+    if (code != 0.0) *ch.stop = 1;
+}
+
 }  // namespace
 
 // ------------------------------------------------------------------ internal API ----
@@ -1159,6 +1298,81 @@ extern "C" int32_t b2k_bicgstab_chain(b2k_ctx* ctx, const b2k_op* op, b2k_vec x,
     for (int32_t i = 0; i < nsteps; ++i)
         if (ctx->h_res[(size_t)B2K_REC * i + 7] != 0.0) { d = i + 1; break; }
     memcpy(rec_out, ctx->h_res, sizeof(double) * B2K_REC * d);
+    *steps_done = d;
+    return B2K_OK;
+}
+
+// Up to `nsteps` MINRES iterations enqueued back to back, two launches each — the SpMV with the 1/beta_k
+// normalisation of its operand applied in the gather and alpha = <v_k, q> in its epilogue, then k_minres_step — and a
+// flush launch that applies the last pending direction / solution update.  ONE host synchronisation per call.
+extern "C" int32_t b2k_minres_chain(b2k_ctx* ctx, const b2k_op* op, b2k_vec x, b2k_vec p_prev, b2k_vec p_cur, b2k_vec q,
+                                    b2k_vec d1, b2k_vec d2, double a0, double a1, const double* state_in, double tol,
+                                    int32_t nsteps, double* rec_out, double* state_out, int32_t* steps_done) {
+    if (!ctx || !op || !state_in || !rec_out || !state_out || !steps_done || nsteps < 1) return B2K_EINVAL;
+    if (nsteps > B2K_MAX_CHAIN - 1) nsteps = B2K_MAX_CHAIN - 1;
+    const b2k_vec hv[6] = {x, p_prev, p_cur, q, d1, d2};
+    VecRef r[6];
+    for (int i = 0; i < 6; ++i) B2K_TRY(b2k_resolve(ctx, hv[i], &r[i]));
+    const int64_t n = r[0].n;
+    int64_t orows = 0, ocols = 0;
+    int32_t okind = -1;
+    B2K_TRY(b2k_op_info(op, &orows, &ocols, nullptr, &okind));
+    if (ctx->nranks > 1) return b2k_fail(ctx, B2K_ENOTSUP, "minres_chain: single-GPU contexts only");
+    if (okind == 1) return b2k_fail(ctx, B2K_ENOTSUP, "minres_chain: CSR / stencil operators only");
+    for (int i = 0; i < 6; ++i)
+        if (r[i].n != n || orows != n || ocols != n) return b2k_fail(ctx, B2K_EDIM, "minres_chain: length mismatch");
+    for (int i = 0; i < 6; ++i)
+        for (int j = 0; j < i; ++j)
+            if (r[i].ptr == r[j].ptr) return b2k_fail(ctx, B2K_EINVAL, "minres_chain: vectors %d and %d are the same", j, i);
+    *steps_done = 0;
+    double* st = ctx->d_steps;
+    double* rec0 = ctx->d_steps + MR_NSTATE;
+    int* d_stop = reinterpret_cast<int*>(ctx->d_sync + B2K_SYNC_STOP);
+    double seed[MR_NSTATE] = {};
+    memcpy(seed, state_in, 8 * sizeof(double));
+    B2K_TRY(b2k_put_coef(ctx, seed, MR_NSTATE, 0));
+    B2K_CUDA(ctx, cudaMemcpyAsync(st, ctx->d_coef, MR_NSTATE * sizeof(double), cudaMemcpyDeviceToDevice, ctx->stream));
+    B2K_CUDA(ctx, cudaMemsetAsync(rec0, 0, sizeof(double) * B2K_REC * nsteps, ctx->stream));
+    B2K_CUDA(ctx, cudaMemsetAsync(d_stop, 0, sizeof(int), ctx->stream));
+    const bool shifted = (a0 != 0.0) || (a1 != 1.0);
+    const int grid = grid_for(ctx, n, 4);
+    const bool f64 = ctx->dtype == B2K_F64;
+    SpmvFuse fz;
+    memset(&fz, 0, sizeof(fz));
+    fz.stop = d_stop;
+    fz.xscale = st + MR_INVB;
+    fz.dot_self = 1;
+    MinresChain ch;
+    ch.st = st; ch.stop = d_stop; ch.alpha = ctx->d_res; ch.tol = tol;
+#define LAUNCH(T, LZ)                                                                                       \
+    k_minres_step<T, LZ><<<grid, BT, 0, ctx->stream>>>((T*)r[0].ptr, (T*)r[1].ptr, (T*)r[2].ptr,            \
+                                                       (const T*)r[3].ptr, (T*)r[4].ptr, (T*)r[5].ptr, n,   \
+                                                       ctx->d_part_s, ctx->d_sync, ch)
+    for (int32_t i = 0; i <= nsteps; ++i) {
+        ch.rec = rec0 + (size_t)B2K_REC * i;
+        if (i == nsteps) {                         // flush
+            if (f64) LAUNCH(double, false);
+            else LAUNCH(float, false);
+        } else {
+            // the operand is p_cur of this iteration: the roles swap with every iteration that runs, and a launch
+            // behind a raised stop flag does nothing, so the host's count is the device's whenever it matters
+            B2K_TRY(b2k_enqueue_apply_fused(ctx, op, r[(i & 1) ? 1 : 2], r[3], a0, a1, shifted, nullptr, ctx->d_res, &fz));
+            if (f64) LAUNCH(double, true);
+            else LAUNCH(float, true);
+        }
+        B2K_LAUNCH_CHECK(ctx);
+    }
+#undef LAUNCH
+    // state and records are one block of d_steps
+    B2K_CUDA(ctx, cudaMemcpyAsync(ctx->h_res, st, sizeof(double) * (MR_NSTATE + B2K_REC * nsteps), cudaMemcpyDeviceToHost,
+                                  ctx->stream));
+    B2K_TRY(b2k_stream_sync(ctx));
+    const double* hrec = ctx->h_res + MR_NSTATE;
+    int32_t d = nsteps;
+    for (int32_t i = 0; i < nsteps; ++i)
+        if (hrec[(size_t)B2K_REC * i + 5] != 0.0) { d = i + 1; break; }
+    memcpy(rec_out, hrec, sizeof(double) * B2K_REC * d);
+    memcpy(state_out, ctx->h_res, 8 * sizeof(double));
     *steps_done = d;
     return B2K_OK;
 }

@@ -181,7 +181,8 @@ __device__ __forceinline__ void b2k_trace(unsigned long long* tr, unsigned code)
 
 // Optional fusions of the Lanczos step into the SpMV (basis.cu, b2k_lanczos_expand_many):
 //   xscale   : device scalar; the operand is x*(*xscale) — the normalisation v = r/β of lanczos.jl:257 applied
-//              while gathering (each gathered entry is rounded exactly like the separate scale!! pass);
+//              while gathering (each gathered entry is rounded exactly like the separate scale!! pass); the a0 term
+//              of a shifted apply multiplies the normalised entry as well;
 //   vout     : the normalised operand is also written out (row r writes x[r]*(*xscale)): it becomes the new
 //              basis vector, in a column of its own because other CTAs still gather the unscaled x;
 //   dot_self : the fused dot product is <x*(*xscale), y> (no separate read of the normalised vector);

@@ -131,7 +131,7 @@ k_spmv_stream(const int32_t* __restrict__ rowptr, const int32_t* __restrict__ co
             const int a = rowptr[r] - p0, b = rowptr[r + 1] - p0;
             T s = (T)0;
             for (int p = a; p < b; ++p) s += prod[p];
-            if (shifted) s = fma(a0, xs[r], a1 * s);
+            if (shifted) s = fma(a0, xs[r] * sc, a1 * s);      // the shift acts on the normalised operand
             y[r] = s;
             T dv = (T)0;
             if (vout || fz.dot_self) {
@@ -157,7 +157,7 @@ k_spmv_stream(const int32_t* __restrict__ rowptr, const int32_t* __restrict__ co
         const double tot = block_sum(acc, red);
         if (tid == 0) {
             T s = (T)tot;
-            if (shifted) s = fma(a0, xs[r0], a1 * s);
+            if (shifted) s = fma(a0, xs[r0] * sc, a1 * s);
             y[r0] = s;
             T dv = (T)0;
             if (vout || fz.dot_self) {
@@ -357,7 +357,7 @@ k_spmv_pipe(const int32_t* __restrict__ rowptr, const int32_t* __restrict__ coli
                 a -= p0a; b -= p0a;
                 T sum = (T)0;
                 for (int p = a; p < b; ++p) sum += vs[p];
-                if (shifted) sum = fma(a0, xsr, a1 * sum);
+                if (shifted) sum = fma(a0, xsr * sc, a1 * sum);      // the shift acts on the normalised operand
                 if (fz.l2_hints) st_hint(y + r, sum, pol_last);
                 else y[r] = sum;
                 if (self) {
@@ -382,7 +382,7 @@ k_spmv_pipe(const int32_t* __restrict__ rowptr, const int32_t* __restrict__ coli
                 double tot = 0.0;
                 for (int i = 0; i < SPP_CONS / 32; ++i) tot += red[i];
                 T sum = (T)tot;
-                if (shifted) sum = fma(a0, xs[r0], a1 * sum);
+                if (shifted) sum = fma(a0, xs[r0] * sc, a1 * sum);
                 y[r0] = sum;
                 T dv = (dotv && !fz.dot_self) ? dotv[r0] : (T)0;
                 if (self) {
@@ -617,7 +617,7 @@ k_spmv_compact(const int32_t* __restrict__ rowptr, const int32_t* __restrict__ c
                 }
                 T sum = (T)0;
                 for (int p = a; p < b; ++p) sum += pr[p];
-                if (shifted) sum = fma(a0, xsr, a1 * sum);
+                if (shifted) sum = fma(a0, xsr * sc, a1 * sum);      // the shift acts on the normalised operand
                 if (fz.l2_hints) st_hint(y + r, sum, pol_last);
                 else y[r] = sum;
                 if (self) {
@@ -641,7 +641,7 @@ k_spmv_compact(const int32_t* __restrict__ rowptr, const int32_t* __restrict__ c
                 double tot = 0.0;
                 for (int i = 0; i < SPP_CONS / 32; ++i) tot += red[i];
                 T sum = (T)tot;
-                if (shifted) sum = fma(a0, xs[r0], a1 * sum);
+                if (shifted) sum = fma(a0, xs[r0] * sc, a1 * sum);
                 y[r0] = sum;
                 T dv = (dotv && !fz.dot_self) ? dotv[r0] : (T)0;
                 if (self) {
@@ -1194,7 +1194,7 @@ k_stencil_apply(const __grid_constant__ StencilApply sa, const T* __restrict__ x
         if (ix < sa.nx - 1) sum = add_rn<T>(sum, mul_rn<T>(ce, X(i + 1)));
         if (iy < sa.ny - 1) sum = add_rn<T>(sum, mul_rn<T>(cn, X(i + sa.nx)));
         if (sa.nz > 1 && iz < sa.nz - 1) sum = add_rn<T>(sum, mul_rn<T>(cu, X(i + plane)));
-        if (shifted) sum = fma(a0, __ldg(x + i), a1 * sum);
+        if (shifted) sum = fma(a0, xi, a1 * sum);      // xi = x_i, normalised when the operand is
         return sum;
     };
     auto finish = [&](int64_t i, T sum, T xi) {

@@ -7,7 +7,7 @@ import warnings
 
 import numpy as np
 
-from .algorithms import BiCGStab, CG, ConvergenceInfo, GMRES, WARN_LEVEL
+from .algorithms import BiCGStab, CG, ConvergenceInfo, GMRES, MINRES, WARN_LEVEL
 from .dense import givens, ldiv_upper
 from .factorizations import arnoldi as ar
 from .operators import B200CSR, apply
@@ -30,7 +30,7 @@ def linsolve(A, b, x0=None, alg: GMRES | None = None, a0: float = 0.0, a1: float
         atol = rtol = None                              # already folded into alg.tol
     elif kwargs:
         raise TypeError(f"linsolve: keyword arguments {sorted(kwargs)} only apply when no algorithm is passed")
-    if isinstance(alg, (CG, BiCGStab)) and not isinstance(b, B200Vec):
+    if isinstance(alg, (CG, BiCGStab, MINRES)) and not isinstance(b, B200Vec):
         return _linsolve_host(A, b, x0, alg, a0, a1, atol, rtol)
     if isinstance(alg, CG):
         if not isinstance(b, B200Vec):
@@ -38,6 +38,10 @@ def linsolve(A, b, x0=None, alg: GMRES | None = None, a0: float = 0.0, a1: float
         if atol is not None or rtol is not None:
             alg = CG(maxiter=alg.maxiter, tol=max(atol or 0.0, (rtol or 0.0) * b.norm()), verbosity=alg.verbosity)
         return _cg(A, b, x0 if x0 is not None else b.zerovector(), alg, a0, a1)
+    if isinstance(alg, MINRES):
+        if atol is not None or rtol is not None:
+            alg = MINRES(maxiter=alg.maxiter, tol=max(atol or 0.0, (rtol or 0.0) * b.norm()), verbosity=alg.verbosity)
+        return _minres(A, b, x0 if x0 is not None else b.zerovector(), alg, a0, a1)
     if isinstance(alg, BiCGStab):
         if not isinstance(b, B200Vec):
             raise TypeError("linsolve(BiCGStab): pass device vectors (B200Vec)")
@@ -431,3 +435,115 @@ def _bicgstab(operator, b: B200Vec, x0: B200Vec, alg: BiCGStab, a0: float, a1: f
                 warnings.warn(f"BiCGStab linsolve stopped without converging after {numiter} iterations: "
                               f"normres = {normr}, numops = {numops}")
             return x, ConvergenceInfo(0, r, normr, numiter, numops)
+
+
+USE_MINRES_CHAIN = True   # b2k_minres_chain: two launches per iteration, one host round trip per MINRES_CHAIN_LEN
+MINRES_CHAIN_LEN = 32
+
+
+def _minres_scalars(st, alpha: float, beta_new: float):
+    """The Givens-QR half of one MINRES iteration, in the operation order of k_minres_step's last CTA (plain double
+    arithmetic, every product and sum rounded on its own).  st = [β_k, 1/β_k, 1/β_{k-1}, c, s, δ̄, ε, φ̄] is advanced
+    in place; returns the record (α, β_{k+1}, γ, φ, |φ̄|, stop code, δ, ε_k)."""
+    c0, s0, dbar, eps, phibar = st[3], st[4], st[5], st[6], st[7]
+    delta = c0 * dbar + s0 * alpha
+    gbar = s0 * dbar - c0 * alpha
+    gamma = math.sqrt(gbar * gbar + beta_new * beta_new)
+    sing = gamma == 0.0
+    c, s = (0.0, 0.0) if sing else (gbar / gamma, beta_new / gamma)
+    phi = 0.0 if sing else c * phibar
+    phibar_n = phibar if sing else s * phibar
+    st[2], st[0], st[1] = st[1], beta_new, (1.0 / beta_new if beta_new != 0.0 else math.inf)
+    st[3], st[4], st[5], st[6], st[7] = c, s, -(c0 * beta_new), s0 * beta_new, phibar_n
+    return alpha, beta_new, gamma, phi, abs(phibar_n), (2.0 if sing else 0.0), delta, eps
+
+
+def _minres(operator, b: B200Vec, x0: B200Vec, alg: MINRES, a0: float, a1: float):
+    """linsolve(operator, b, x₀, alg::MINRES, a₀, a₁) for a real symmetric operator that need not be definite.  The
+    reference declares the algorithm (src/algorithms.jl:397-427) and leaves the driver as a TODO
+    (src/linsolve/linsolve.jl:140-141), so the recurrence is fixed here: Paige & Saunders (1975), unpreconditioned
+    Lanczos + Givens QR, with the stopping rules of cg.jl:69-73 (a recurrence residual is never trusted: when |φ̄|
+    < tol the residual is computed, and if it is not below tol the process restarts from the current x).
+    A device CSR operator on one GPU runs b2k_minres_chain (the Lanczos vectors stay unnormalised, two launches
+    per iteration, one host round trip per MINRES_CHAIN_LEN iterations); every other operator, and row-sharded
+    contexts, run the literal VectorInterface sequence, which produces the same vectors given the same scalars."""
+    import ctypes as C
+    y0 = apply(operator, x0)
+    r = b.copy()
+    if a0 != 0:
+        r = r.add_(x0, -a0)
+    r = r.add_(y0, -a1)
+    del y0
+    x = x0.copy()
+    normr = r.norm()
+    maxiter, tol = alg.maxiter, alg.tol
+    numops, numiter = 1, 0
+    if normr < tol:
+        return x, ConvergenceInfo(1, r, normr, numiter, numops)
+    ctx = b.ctx
+    chain = USE_MINRES_CHAIN and isinstance(operator, B200CSR) and ctx.nranks == 1
+    d1, d2 = r.zerovector(), r.zerovector()
+    if chain:       # p_cur = p_{k-1}, p_prev = p_{k-2}: the Lanczos vectors before normalisation (v_k = p_{k-1}/β_k)
+        p_cur, p_prev, q = r.copy(), r.zerovector(), r.zerovector()
+    else:
+        v, v_prev = r.scale(1.0 / normr), r.zerovector()
+    st = [normr, 1.0 / normr, 0.0, -1.0, 0.0, 0.0, 0.0, normr]
+    pending: list = []            # records of iterations the device has already run, oldest first
+    while True:
+        if chain:
+            if not pending:
+                m = max(1, min(MINRES_CHAIN_LEN, maxiter - numiter))
+                rec, done = np.zeros((m, 8)), C.c_int32()
+                sin, sout = (C.c_double * 8)(*st), (C.c_double * 8)()
+                ctx.check(ctx.lib.b2k_minres_chain(ctx.h, operator.h, x.handle, p_prev.handle, p_cur.handle, q.handle,
+                                                   d1.handle, d2.handle, a0, a1, sin, tol, m,
+                                                   rec.ctypes.data_as(C.POINTER(C.c_double)), sout, C.byref(done)))
+                st = list(sout)
+                if done.value & 1:                                   # the roles rotate once per iteration
+                    p_prev, p_cur, d1, d2 = p_cur, p_prev, d2, d1
+                pending = [rec[i] for i in range(done.value)]
+            _, beta_new, gamma, _, phibar, _, _, _ = pending.pop(0)
+        else:
+            q = apply(operator, v, a0, a1)
+            alpha = v.inner(q)
+            q = q.add_(v, -alpha)
+            q = q.add_(v_prev, -st[0])
+            eps = st[6]
+            _, beta_new, gamma, phi, phibar, _, delta, _ = _minres_scalars(st, alpha, q.norm())
+            d = v_prev.scale_(1.0, v)                                # v_{k-1} has done its work: d_k takes its storage
+            if gamma != 0.0:
+                d = d.add_(d1, -delta)
+                d = d.add_(d2, -eps)
+                d = d.scale_(1.0 / gamma)
+                x = x.add_(d, phi)
+            else:
+                d = d.zerovector_()
+            d1, d2, v_prev = d, d1, v
+            v = q.scale_(st[1]) if beta_new != 0.0 else q            # v_{k+1} = p_k/β_{k+1}
+        numiter += 1
+        numops += 1
+        hit = phibar < tol or beta_new == 0.0
+        if gamma == 0.0 or hit or numiter >= maxiter:
+            r = r.scale_(1.0, b)
+            r = r.add_(apply(operator, x, a0, a1), -1.0)
+            numops += 1
+            normr = r.norm()
+            if gamma == 0.0:
+                if alg.verbosity >= WARN_LEVEL:
+                    warnings.warn(f"MINRES linsolve in iteration {numiter}: the operator is singular in the Krylov "
+                                  f"subspace: normres = {normr}, numops = {numops}")
+                return x, ConvergenceInfo(0, r, normr, numiter, numops)
+            if hit and (normr < tol or normr == 0.0):               # (tol = 0: an exact solution still ends it)
+                return x, ConvergenceInfo(1, r, normr, numiter, numops)
+            if numiter >= maxiter:
+                if alg.verbosity >= WARN_LEVEL:
+                    warnings.warn(f"MINRES linsolve stopped without converging after {numiter} iterations: "
+                                  f"normres = {normr}, numops = {numops}")
+                return x, ConvergenceInfo(0, r, normr, numiter, numops)
+            # the recurrence reported convergence and the residual does not confirm it: a fresh process from x
+            if chain:
+                p_cur, p_prev = p_cur.scale_(1.0, r), p_prev.zerovector_()
+            else:
+                v, v_prev = v.scale_(1.0 / normr, r), v_prev.zerovector_()
+            d1, d2 = d1.zerovector_(), d2.zerovector_()
+            st = [normr, 1.0 / normr, 0.0, -1.0, 0.0, 0.0, 0.0, normr]
