@@ -288,24 +288,10 @@ k_dot(const T* __restrict__ q, T* __restrict__ x, int64_t n, const T* __restrict
         }
         acc = NORM ? fma(b, b, acc) : fma(q[i], b, acc);
     }
-    double s = block_sum((double)acc, red);
-    if (threadIdx.x == 0) {
-        part[blockIdx.x] = s;
-        __threadfence();
-        unsigned t = atomicInc(ticket, gridDim.x - 1);
-        last = (t == gridDim.x - 1);
-    }
-    __syncthreads();
-    if (last) {
-        __threadfence();
-        double v = 0.0;
-        for (int g = threadIdx.x; g < gridDim.x; g += BT) v += part[g];   // fixed assignment
-        double tot = block_sum(v, red);
-        if (threadIdx.x == 0) {
-            *out = tot;
-            if (accum_into) *accum_into += tot;
-        }
-    }
+    finish_sums<1>({block_sum((double)acc, red)}, part, ticket, red, &last, BT, [&](int, double tot) {
+        *out = tot;
+        if (accum_into) *accum_into += tot;
+    });
 }
 
 // final fix-up: x <- x - s*q with s = d_res[src] (tail of the pipelined MGS sweep)
@@ -376,34 +362,19 @@ k_cg_xr(T* __restrict__ x, T* __restrict__ r, const T* __restrict__ p, const T* 
         r[i] = rr;
         acc = fma(rr, rr, acc);
     }
-    const double sblk = block_sum((double)acc, red);
-    if (threadIdx.x == 0) {
-        part[blockIdx.x] = sblk;
-        __threadfence();
-        const unsigned t = atomicInc(ticket, gridDim.x - 1);
-        last = (t == gridDim.x - 1);
-    }
-    __syncthreads();
-    if (last) {
-        __threadfence();
-        double v = 0.0;
-        const volatile double* pv2 = part;
-        for (int g = threadIdx.x; g < (int)gridDim.x; g += BT) v += pv2[g];
-        const double tot = block_sum(v, red);
-        if (threadIdx.x == 0) {
-            *out = tot;
-            if (ch.state) {
-                // cg.jl:74-77 on the device: normr = sqrt(||r||^2); rho_old = rho; rho = normr^2; beta = rho / rho_old
-                const double nr = sqrt(tot);
-                const double rho_new = nr * nr;
-                ch.state[1] = rho_new / rho;
-                ch.state[0] = rho_new;
-                ch.rec[0] = *pq;
-                ch.rec[1] = nr;
-                if (nr < ch.tol) *ch.stop = 1;     // cg.jl:68: the host takes over (explicit residual, restart)
-            }
+    finish_sums<1>({block_sum((double)acc, red)}, part, ticket, red, &last, BT, [&](int, double tot) {
+        *out = tot;
+        if (ch.state) {
+            // cg.jl:74-77 on the device: normr = sqrt(||r||^2); rho_old = rho; rho = normr^2; beta = rho / rho_old
+            const double nr = sqrt(tot);
+            const double rho_new = nr * nr;
+            ch.state[1] = rho_new / rho;
+            ch.state[0] = rho_new;
+            ch.rec[0] = *pq;
+            ch.rec[1] = nr;
+            if (nr < ch.tol) *ch.stop = 1;     // cg.jl:68: the host takes over (explicit residual, restart)
         }
-    }
+    });
 }
 
 // x + beta*y with the product rounded first: what k_axpby<T, 2> computes for alpha = 1, fma(1, x, rn(beta*y)).
@@ -479,33 +450,6 @@ k_bicg_p(T* __restrict__ p, const T* __restrict__ r, const T* __restrict__ v, in
     }
 }
 
-// two-stage deterministic finish shared by the kernels below: per-CTA partials, last CTA adds them in
-// CTA order; NRED independent sums (part is NRED x gridDim.x)
-template <int NRED>
-__device__ __forceinline__ void finish_sums(const double (&blk)[NRED], double* __restrict__ part,
-                                            unsigned* __restrict__ ticket, double* __restrict__ out,
-                                            double* red, bool* last) {
-    if (threadIdx.x == 0) {
-#pragma unroll
-        for (int k = 0; k < NRED; ++k) part[(size_t)k * gridDim.x + blockIdx.x] = blk[k];
-        __threadfence();
-        const unsigned t = atomicInc(ticket, gridDim.x - 1);
-        *last = (t == gridDim.x - 1);
-    }
-    __syncthreads();
-    if (*last) {
-        __threadfence();
-        const volatile double* pv = part;
-#pragma unroll
-        for (int k = 0; k < NRED; ++k) {
-            double v = 0.0;
-            for (int g = threadIdx.x; g < (int)gridDim.x; g += BT) v += pv[(size_t)k * gridDim.x + g];
-            const double tot = block_sum(v, red);
-            if (threadIdx.x == 0) out[k] = tot;
-        }
-    }
-}
-
 // s <- r - alpha*v with alpha = rho / *sigma (device scalar); out[0] = ||s||^2   (bicgstab.jl:109-116)
 template <typename T>
 __global__ void __launch_bounds__(BT)
@@ -542,8 +486,7 @@ k_bicg_s(T* __restrict__ s, const T* __restrict__ r, const T* __restrict__ v, in
         s[i] = sv;
         acc = fma(sv, sv, acc);
     }
-    const double blk[1] = {block_sum((double)acc, red)};
-    finish_sums<1>(blk, part, ticket, out, red, &last);
+    finish_sums<1>({block_sum((double)acc, red)}, part, ticket, red, &last, BT, [&](int k, double tot) { out[k] = tot; });
     if (ch.st && last && threadIdx.x == 0) {
         // bicgstab.jl:106-118 on the device: alpha = rho / sigma, the half-step residual norm and its test
         const double sg = *sigma, al = rho / sg, ns = sqrt(out[0]);
@@ -605,7 +548,7 @@ k_bicg_xr(T* __restrict__ x, T* __restrict__ r, const T* __restrict__ rs, const 
     double blk[2];
     blk[0] = block_sum((double)a1, red);
     blk[1] = block_sum((double)a2, red);
-    finish_sums<2>(blk, part, ticket, out, red, &last);
+    finish_sums<2>(blk, part, ticket, red, &last, BT, [&](int k, double tot) { out[k] = tot; });
     if (ch.st && last && threadIdx.x == 0) {
         // bicgstab.jl:141-152 and the next iteration's :97-98 on the device
         const double om = *ts / *tt, nr = sqrt(out[0]), rho_next = out[1];
@@ -715,48 +658,35 @@ k_minres_step(T* __restrict__ x, T* pA, T* pB, const T* __restrict__ q, T* dA, T
         }
     }
     if (!LANCZOS) return;
-    const double sblk = block_sum((double)acc, red);
-    if (threadIdx.x == 0) {
-        part[blockIdx.x] = sblk;
-        __threadfence();
-        const unsigned t = atomicInc(ticket, gridDim.x - 1);
-        last = (t == gridDim.x - 1);
-    }
-    __syncthreads();
-    if (!last) return;
-    __threadfence();
-    double v = 0.0;
-    const volatile double* pv2 = part;
-    for (int g = threadIdx.x; g < (int)gridDim.x; g += BT) v += pv2[g];
-    const double tot = block_sum(v, red);
-    if (threadIdx.x != 0) return;
-    const double bn = sqrt(tot);                                        // beta_{k+1}
-    const double c0 = st[MR_C], s0 = st[MR_S], dbar = st[MR_DBAR], eps = st[MR_EPS], phibar = st[MR_PHIBAR];
-    const double delta = __dadd_rn(__dmul_rn(c0, dbar), __dmul_rn(s0, alpha));
-    const double gbar = __dadd_rn(__dmul_rn(s0, dbar), -__dmul_rn(c0, alpha));
-    const double gamma = sqrt(__dadd_rn(__dmul_rn(gbar, gbar), __dmul_rn(bn, bn)));
-    // gamma == 0: the shifted operator is singular on the Krylov space.  The pending update is kept, with zero
-    // weights (d_k = 0, x unchanged), so the roles rotate the same way on every exit.
-    const bool sing = gamma == 0.0;
-    const double c = sing ? 0.0 : __ddiv_rn(gbar, gamma), s = sing ? 0.0 : __ddiv_rn(bn, gamma);
-    const double phi = sing ? 0.0 : __dmul_rn(c, phibar), phibar_n = sing ? phibar : __dmul_rn(s, phibar);
-    const double code = sing ? 2.0 : (fabs(phibar_n) < ch.tol ? 1.0 : (bn == 0.0 ? 3.0 : 0.0));
-    double* w = ch.st;
-    w[MR_INVB_PREV] = invb;
-    w[MR_BETA] = bn;
-    w[MR_INVB] = __ddiv_rn(1.0, bn);
-    w[MR_C] = c; w[MR_S] = s;
-    w[MR_DBAR] = -__dmul_rn(c0, bn);
-    w[MR_EPS] = __dmul_rn(s0, bn);
-    w[MR_PHIBAR] = phibar_n;
-    w[MR_PDELTA] = delta; w[MR_PEPS] = eps;
-    w[MR_PINVG] = sing ? 0.0 : __ddiv_rn(1.0, gamma);
-    w[MR_PPHI] = phi;
-    w[MR_PEND] = 1.0;
-    w[MR_DONE] = (double)(done + 1);
-    ch.rec[0] = alpha; ch.rec[1] = bn; ch.rec[2] = gamma; ch.rec[3] = phi; ch.rec[4] = fabs(phibar_n);
-    ch.rec[5] = code; ch.rec[6] = delta; ch.rec[7] = eps;
-    if (code != 0.0) *ch.stop = 1;
+    finish_sums<1>({block_sum((double)acc, red)}, part, ticket, red, &last, BT, [&](int, double tot) {
+        const double bn = sqrt(tot);                                        // beta_{k+1}
+        const double c0 = st[MR_C], s0 = st[MR_S], dbar = st[MR_DBAR], eps = st[MR_EPS], phibar = st[MR_PHIBAR];
+        const double delta = __dadd_rn(__dmul_rn(c0, dbar), __dmul_rn(s0, alpha));
+        const double gbar = __dadd_rn(__dmul_rn(s0, dbar), -__dmul_rn(c0, alpha));
+        const double gamma = sqrt(__dadd_rn(__dmul_rn(gbar, gbar), __dmul_rn(bn, bn)));
+        // gamma == 0: the shifted operator is singular on the Krylov space.  The pending update is kept, with zero
+        // weights (d_k = 0, x unchanged), so the roles rotate the same way on every exit.
+        const bool sing = gamma == 0.0;
+        const double c = sing ? 0.0 : __ddiv_rn(gbar, gamma), s = sing ? 0.0 : __ddiv_rn(bn, gamma);
+        const double phi = sing ? 0.0 : __dmul_rn(c, phibar), phibar_n = sing ? phibar : __dmul_rn(s, phibar);
+        const double code = sing ? 2.0 : (fabs(phibar_n) < ch.tol ? 1.0 : (bn == 0.0 ? 3.0 : 0.0));
+        double* w = ch.st;
+        w[MR_INVB_PREV] = invb;
+        w[MR_BETA] = bn;
+        w[MR_INVB] = __ddiv_rn(1.0, bn);
+        w[MR_C] = c; w[MR_S] = s;
+        w[MR_DBAR] = -__dmul_rn(c0, bn);
+        w[MR_EPS] = __dmul_rn(s0, bn);
+        w[MR_PHIBAR] = phibar_n;
+        w[MR_PDELTA] = delta; w[MR_PEPS] = eps;
+        w[MR_PINVG] = sing ? 0.0 : __ddiv_rn(1.0, gamma);
+        w[MR_PPHI] = phi;
+        w[MR_PEND] = 1.0;
+        w[MR_DONE] = (double)(done + 1);
+        ch.rec[0] = alpha; ch.rec[1] = bn; ch.rec[2] = gamma; ch.rec[3] = phi; ch.rec[4] = fabs(phibar_n);
+        ch.rec[5] = code; ch.rec[6] = delta; ch.rec[7] = eps;
+        if (code != 0.0) *ch.stop = 1;
+    });
 }
 
 }  // namespace

@@ -463,6 +463,34 @@ __device__ __forceinline__ double block_sum(double v, double* red) {
     return s;
 }
 
+// Deterministic grid sums, two-stage: each CTA stores its partials blk[k] (block_sum results, valid in thread 0) in
+// part[k * gridDim.x + blockIdx.x], the last CTA to take a ticket adds them in CTA order (thread i taking partials
+// i, i + nt, ..., then block_sum) and its thread 0 calls fin(k, total_k) for k = 0 .. NRED-1 in turn.  Every thread
+// of the block calls it; `last` is a __shared__ flag.
+template <int NRED, typename Fin>
+__device__ __forceinline__ void finish_sums(const double (&blk)[NRED], double* __restrict__ part,
+                                            unsigned* __restrict__ ticket, double* red, bool* last, int nt, Fin fin) {
+    if (threadIdx.x == 0) {
+#pragma unroll
+        for (int k = 0; k < NRED; ++k) part[(size_t)k * gridDim.x + blockIdx.x] = blk[k];
+        __threadfence();
+        const unsigned t = atomicInc(ticket, gridDim.x - 1);
+        *last = (t == gridDim.x - 1);
+    }
+    __syncthreads();
+    if (*last) {
+        __threadfence();
+        const volatile double* pv = part;
+#pragma unroll
+        for (int k = 0; k < NRED; ++k) {
+            double s = 0.0;
+            for (int g = threadIdx.x; g < (int)gridDim.x; g += nt) s += pv[(size_t)k * gridDim.x + g];
+            const double tot = block_sum(s, red);
+            if (threadIdx.x == 0) fin(k, tot);
+        }
+    }
+}
+
 __device__ __forceinline__ uint64_t splitmix64(uint64_t z) {
     z += 0x9E3779B97F4A7C15ull;
     z = (z ^ (z >> 30)) * 0xBF58476D1CE4E5B9ull;

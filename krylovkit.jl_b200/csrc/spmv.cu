@@ -173,25 +173,10 @@ k_spmv_stream(const int32_t* __restrict__ rowptr, const int32_t* __restrict__ co
         }
     }
     if (dotv || fz.dot_self) {
-        const double s = block_sum((double)dacc, red);
-        if (tid == 0) {
-            part[blockIdx.x] = s;
-            __threadfence();
-            const unsigned t = atomicInc(ticket, gridDim.x - 1);
-            last = (t == gridDim.x - 1);
-        }
-        __syncthreads();
-        if (last) {
-            __threadfence();
-            double v2 = 0.0;
-            const volatile double* pv = part;
-            for (int g = tid; g < (int)gridDim.x; g += SP_BT) v2 += pv[g];
-            const double tot = block_sum(v2, red);
-            if (tid == 0) {
-                *out = tot;
-                if (ps.on && ps.seq_alpha) peer_publish1(ps.pd, PEER_CH_ALPHA, ps.seq_alpha, tot);
-            }
-        }
+        finish_sums<1>({block_sum((double)dacc, red)}, part, ticket, red, &last, SP_BT, [&](int, double tot) {
+            *out = tot;
+            if (ps.on && ps.seq_alpha) peer_publish1(ps.pd, PEER_CH_ALPHA, ps.seq_alpha, tot);
+        });
     }
 }
 
@@ -223,6 +208,79 @@ __global__ void k_pblk(const int32_t* __restrict__ rowptr, const int32_t* __rest
     const int b = blockIdx.x * blockDim.x + threadIdx.x;
     if (b < count) pblk[b] = rowptr[rowblk[b]];
 }
+
+// Row epilogue of the single-operator TMA kernels (k_spmv_pipe, k_spmv_compact): y_r = a0 xs_r + a1 (A x)_r with the
+// shift acting on the normalised operand, vout_r = the normalised x_r, and the dot chain dacc = fma(dv_r, y_r - dsc
+// dsub_r, dacc) over the thread's rows, dv = dotv or the normalised x (fz.dot_self).  load(r) issues a row's global
+// loads, before its sum so that they overlap it; row(r, loads, sum) finishes it.
+template <typename T>
+struct RowEpilogue {
+    struct Loads { T dv, xself, xsr, dsv; };
+    const SpmvFuse fz;
+    const T* x;
+    T* y;
+    const T* xs;
+    const T* dotv;
+    T a0, a1;
+    int shifted;
+    bool scaled = fz.xscale != nullptr;
+    T sc = scaled ? (T)(*fz.xscale) : (T)1;
+    T* vout = reinterpret_cast<T*>(fz.vout);
+    bool self = (vout != nullptr) || fz.dot_self;
+    bool want_dot = (dotv != nullptr) || fz.dot_self;
+    uint64_t pol_last = fz.l2_hints ? l2_policy_evict_last() : 0;
+    const T* dsub = reinterpret_cast<const T*>(fz.dot_sub_vec);
+    T dsc = dsub ? (T)(*fz.dot_sub_scale) : (T)0;
+    T dacc = (T)0;
+
+    __device__ __forceinline__ Loads load(int r) const {
+        return {(dotv && !fz.dot_self) ? __ldg(dotv + r) : (T)0, self ? __ldg(x + r) : (T)0,
+                shifted ? __ldg(xs + r) : (T)0, dsub ? __ldg(dsub + r) : (T)0};
+    }
+    __device__ __forceinline__ void row(int r, const Loads& l, T sum) {
+        if (shifted) sum = fma(a0, l.xsr * sc, a1 * sum);      // the shift acts on the normalised operand
+        if (fz.l2_hints) st_hint(y + r, sum, pol_last);
+        else y[r] = sum;
+        T dv = l.dv;
+        if (self) {
+            const T vn = l.xself * sc;
+            if (vout) vout[r] = vn;
+            if (fz.dot_self) dv = vn;
+        }
+        dacc = fma(dv, dsub ? fma(-dsc, l.dsv, sum) : sum, dacc);
+    }
+    // A row of more than SP_NNZ nonzeros, the CTA's only one: a double sum of the rounded products, thread i taking
+    // nonzeros i, i + SPP_CONS, ..., then warp butterflies and the warps in order, rounded to T once.  xg(c) = x_c.
+    template <typename G>
+    __device__ __forceinline__ void long_row(int r0, const T* vals, const int32_t* colidx, int p0, int nnzb,
+                                             double* red, G xg) {
+        const int tid = threadIdx.x, lane = tid & 31, w = tid >> 5;
+        double acc = 0.0;
+        for (int i = tid; i < nnzb; i += SPP_CONS) {
+            T xv = xg(colidx[p0 + i]);
+            if (scaled) xv *= sc;
+            acc += (double)mul_rn<T>(vals[p0 + i], xv);
+        }
+        acc = warp_sum(acc);
+        if (lane == 0) red[w] = acc;
+        named_bar_sync(1, SPP_CONS);
+        if (tid == 0) {
+            double tot = 0.0;
+            for (int i = 0; i < SPP_CONS / 32; ++i) tot += red[i];
+            T sum = (T)tot;
+            if (shifted) sum = fma(a0, xs[r0] * sc, a1 * sum);
+            y[r0] = sum;
+            T dv = (dotv && !fz.dot_self) ? dotv[r0] : (T)0;
+            if (self) {
+                const T vn = __ldg(x + r0) * sc;
+                if (vout) vout[r0] = vn;
+                if (fz.dot_self) dv = vn;
+            }
+            if (want_dot) dacc = fma(dv, dsub ? fma(-dsc, dsub[r0], sum) : sum, dacc);
+        }
+        named_bar_sync(1, SPP_CONS);
+    }
+};
 
 // NSTG ring stages, MINB CTAs per SM (variants: (3, 3); (2, 4): fewer stages, more resident warps to hide the
 // latency of the x gather)
@@ -301,15 +359,7 @@ k_spmv_pipe(const int32_t* __restrict__ rowptr, const int32_t* __restrict__ coli
         named_bar_sync(1, SPP_CONS);
     }
     if (tr0) b2k_trace(fz.trace, 2);
-    const bool scaled = fz.xscale != nullptr;
-    const T sc = scaled ? (T)(*fz.xscale) : (T)1;
-    T* const vout = reinterpret_cast<T*>(fz.vout);
-    const bool self = (vout != nullptr) || fz.dot_self;
-    const bool want_dot = (dotv != nullptr) || fz.dot_self;
-    const uint64_t pol_last = fz.l2_hints ? l2_policy_evict_last() : 0;
-    const T* const dsub = reinterpret_cast<const T*>(fz.dot_sub_vec);
-    const T dsc = dsub ? (T)(*fz.dot_sub_scale) : (T)0;
-    T dacc = (T)0;
+    RowEpilogue<T> ep{fz, x, y, xs, dotv, a0, a1, shifted};
     int tile = blockIdx.x;
     int4 dn = make_int4(0, 0, 0, 0);
     if (tile < nblk) dn = make_int4(rowblk[tile], rowblk[tile + 1], pblk[tile], pblk[tile + 1]);
@@ -334,9 +384,9 @@ k_spmv_pipe(const int32_t* __restrict__ rowptr, const int32_t* __restrict__ coli
                     xv[u] = (cc < n_loc) ? __ldg(x + cc) : __ldg(halo + (cc - n_loc));
                 }
             }
-            if (scaled) {
+            if (ep.scaled) {
 #pragma unroll
-                for (int u = 0; u < U; ++u) xv[u] *= sc;      // v_j = r_j * (1/β), rounded like scale!!
+                for (int u = 0; u < U; ++u) xv[u] *= ep.sc;      // v_j = r_j * (1/β), rounded like scale!!
             }
 #pragma unroll
             for (int u = 0; u < U; ++u) {
@@ -346,53 +396,18 @@ k_spmv_pipe(const int32_t* __restrict__ rowptr, const int32_t* __restrict__ coli
             named_bar_sync(1, SPP_CONS);
             const bool rp_staged = nrows <= SPP_RMAX;
             for (int r = r0 + tid; r < r1; r += SPP_CONS) {
-                // issue the (optional) per-row global loads first so they overlap the row sum
-                T dv = (dotv && !fz.dot_self) ? __ldg(dotv + r) : (T)0;
-                const T xself = self ? __ldg(x + r) : (T)0;
-                const T xsr = shifted ? __ldg(xs + r) : (T)0;
-                const T dsv = dsub ? __ldg(dsub + r) : (T)0;
+                const auto ld = ep.load(r);
                 int a, b;
                 if (rp_staged) { a = rs[r - r0a]; b = rs[r + 1 - r0a]; }
                 else { a = rowptr[r]; b = rowptr[r + 1]; }
                 a -= p0a; b -= p0a;
                 T sum = (T)0;
                 for (int p = a; p < b; ++p) sum += vs[p];
-                if (shifted) sum = fma(a0, xsr * sc, a1 * sum);      // the shift acts on the normalised operand
-                if (fz.l2_hints) st_hint(y + r, sum, pol_last);
-                else y[r] = sum;
-                if (self) {
-                    const T vn = xself * sc;
-                    if (vout) vout[r] = vn;
-                    if (fz.dot_self) dv = vn;
-                }
-                dacc = fma(dv, dsub ? fma(-dsc, dsv, sum) : sum, dacc);
+                ep.row(r, ld, sum);
             }
         } else {
-            double acc = 0.0;
-            for (int i = tid; i < nnzb; i += SPP_CONS) {
-                const int32_t cc = colidx[p0 + i];
-                T xv = (cc < n_loc) ? __ldg(x + cc) : __ldg(halo + (cc - n_loc));
-                if (scaled) xv *= sc;
-                acc += (double)mul_rn<T>(vals[p0 + i], xv);
-            }
-            acc = warp_sum(acc);
-            if (lane == 0) red[w] = acc;
-            named_bar_sync(1, SPP_CONS);
-            if (tid == 0) {
-                double tot = 0.0;
-                for (int i = 0; i < SPP_CONS / 32; ++i) tot += red[i];
-                T sum = (T)tot;
-                if (shifted) sum = fma(a0, xs[r0] * sc, a1 * sum);
-                y[r0] = sum;
-                T dv = (dotv && !fz.dot_self) ? dotv[r0] : (T)0;
-                if (self) {
-                    const T vn = __ldg(x + r0) * sc;
-                    if (vout) vout[r0] = vn;
-                    if (fz.dot_self) dv = vn;
-                }
-                if (want_dot) dacc = fma(dv, dsub ? fma(-dsc, dsub[r0], sum) : sum, dacc);
-            }
-            named_bar_sync(1, SPP_CONS);
+            ep.long_row(r0, vals, colidx, p0, nnzb, red,
+                        [&](int32_t cc) { return (cc < n_loc) ? __ldg(x + cc) : __ldg(halo + (cc - n_loc)); });
         }
         fence_proxy_async();   // generic-proxy writes to the stage precede its reuse by the TMA unit
         __syncwarp();
@@ -400,8 +415,8 @@ k_spmv_pipe(const int32_t* __restrict__ rowptr, const int32_t* __restrict__ coli
         if (++s == NSTG) { s = 0; ph ^= 1; }
     }
     if (tr0) b2k_trace(fz.trace, 3);
-    if (want_dot) {
-        double v = warp_sum((double)dacc);
+    if (ep.want_dot) {
+        double v = warp_sum((double)ep.dacc);
         if (lane == 0) red[w] = v;
         named_bar_sync(1, SPP_CONS);
         if (tid == 0) {
@@ -536,15 +551,7 @@ k_spmv_compact(const int32_t* __restrict__ rowptr, const int32_t* __restrict__ c
     const bool tr0 = fz.trace && blockIdx.x == 0 && tid == 0;
     if (tr0) b2k_trace(fz.trace, 1);
     if (tr0) b2k_trace(fz.trace, 2);
-    const bool scaled = fz.xscale != nullptr;
-    const T sc = scaled ? (T)(*fz.xscale) : (T)1;
-    T* const vout = reinterpret_cast<T*>(fz.vout);
-    const bool self = (vout != nullptr) || fz.dot_self;
-    const bool want_dot = (dotv != nullptr) || fz.dot_self;
-    const uint64_t pol_last = fz.l2_hints ? l2_policy_evict_last() : 0;
-    const T* const dsub = reinterpret_cast<const T*>(fz.dot_sub_vec);
-    const T dsc = dsub ? (T)(*fz.dot_sub_scale) : (T)0;
-    T dacc = (T)0;
+    RowEpilogue<T> ep{fz, x, y, xs, dotv, a0, a1, shifted};
     // The x gather of the next tile is issued before the row sums of this one, so its latency (the first touch of an
     // entry of x misses L2) overlaps them instead of stalling the CTA once per tile.
     constexpr int U = SP_NNZ / SPP_CONS;
@@ -583,9 +590,9 @@ k_spmv_compact(const int32_t* __restrict__ rowptr, const int32_t* __restrict__ c
             VS* vs = reinterpret_cast<VS*>(st);
             const uint16_t* rs = reinterpret_cast<const uint16_t*>(st + LY::VAL_BYTES + LY::COL_BYTES);
             const int offv = p0 - al_dn<VS>(p0), r0a = al_dn<uint16_t>(r0);
-            if (scaled) {
+            if (ep.scaled) {
 #pragma unroll
-                for (int u = 0; u < U; ++u) xv[u] *= sc;      // v_j = r_j * (1/β), rounded like scale!!
+                for (int u = 0; u < U; ++u) xv[u] *= ep.sc;      // v_j = r_j * (1/β), rounded like scale!!
             }
             T* pr;
             if constexpr (LY::PROD) {
@@ -603,10 +610,7 @@ k_spmv_compact(const int32_t* __restrict__ rowptr, const int32_t* __restrict__ c
             prefetch_next();
             const bool rp_staged = nrows <= SPP_RMAX;
             for (int r = r0 + tid; r < r1; r += SPP_CONS) {
-                T dv = (dotv && !fz.dot_self) ? __ldg(dotv + r) : (T)0;
-                const T xself = self ? __ldg(x + r) : (T)0;
-                const T xsr = shifted ? __ldg(xs + r) : (T)0;
-                const T dsv = dsub ? __ldg(dsub + r) : (T)0;
+                const auto ld = ep.load(r);
                 int a, b;
                 if (rp_staged) {
                     a = (uint16_t)(rs[r - r0a] - (uint16_t)p0);
@@ -617,41 +621,10 @@ k_spmv_compact(const int32_t* __restrict__ rowptr, const int32_t* __restrict__ c
                 }
                 T sum = (T)0;
                 for (int p = a; p < b; ++p) sum += pr[p];
-                if (shifted) sum = fma(a0, xsr * sc, a1 * sum);      // the shift acts on the normalised operand
-                if (fz.l2_hints) st_hint(y + r, sum, pol_last);
-                else y[r] = sum;
-                if (self) {
-                    const T vn = xself * sc;
-                    if (vout) vout[r] = vn;
-                    if (fz.dot_self) dv = vn;
-                }
-                dacc = fma(dv, dsub ? fma(-dsc, dsv, sum) : sum, dacc);
+                ep.row(r, ld, sum);
             }
         } else {
-            double acc = 0.0;
-            for (int i = tid; i < nnzb; i += SPP_CONS) {
-                T xl = __ldg(x + colidx[p0 + i]);
-                if (scaled) xl *= sc;
-                acc += (double)mul_rn<T>(vals[p0 + i], xl);
-            }
-            acc = warp_sum(acc);
-            if (lane == 0) red[w] = acc;
-            named_bar_sync(1, SPP_CONS);
-            if (tid == 0) {
-                double tot = 0.0;
-                for (int i = 0; i < SPP_CONS / 32; ++i) tot += red[i];
-                T sum = (T)tot;
-                if (shifted) sum = fma(a0, xs[r0] * sc, a1 * sum);
-                y[r0] = sum;
-                T dv = (dotv && !fz.dot_self) ? dotv[r0] : (T)0;
-                if (self) {
-                    const T vn = __ldg(x + r0) * sc;
-                    if (vout) vout[r0] = vn;
-                    if (fz.dot_self) dv = vn;
-                }
-                if (want_dot) dacc = fma(dv, dsub ? fma(-dsc, dsub[r0], sum) : sum, dacc);
-            }
-            named_bar_sync(1, SPP_CONS);
+            ep.long_row(r0, vals, colidx, p0, nnzb, red, [&](int32_t c) { return __ldg(x + c); });
             prefetch_next();
         }
         fence_proxy_async();   // generic-proxy writes to the stage precede its reuse by the TMA unit
@@ -661,8 +634,8 @@ k_spmv_compact(const int32_t* __restrict__ rowptr, const int32_t* __restrict__ c
         ph = ph1;
     }
     if (tr0) b2k_trace(fz.trace, 3);
-    if (want_dot) {
-        double v = warp_sum((double)dacc);
+    if (ep.want_dot) {
+        double v = warp_sum((double)ep.dacc);
         if (lane == 0) red[w] = v;
         named_bar_sync(1, SPP_CONS);
         if (tid == 0) {
@@ -1218,25 +1191,10 @@ k_stencil_apply(const __grid_constant__ StencilApply sa, const T* __restrict__ x
         if (two) finish(i2, sb_, xb);
     }
     if (want_dot) {
-        const double sblk = block_sum((double)dacc, red);
-        if (threadIdx.x == 0) {
-            part[blockIdx.x] = sblk;
-            __threadfence();
-            const unsigned t = atomicInc(ticket, gridDim.x - 1);
-            last = (t == gridDim.x - 1);
-        }
-        __syncthreads();
-        if (last) {
-            __threadfence();
-            double v2 = 0.0;
-            const volatile double* pv = part;
-            for (int gidx = threadIdx.x; gidx < (int)gridDim.x; gidx += blockDim.x) v2 += pv[gidx];
-            const double tot = block_sum(v2, red);
-            if (threadIdx.x == 0) {
-                *out = tot;
-                if (ps.on && ps.seq_alpha) peer_publish1(ps.pd, PEER_CH_ALPHA, ps.seq_alpha, tot);
-            }
-        }
+        finish_sums<1>({block_sum((double)dacc, red)}, part, ticket, red, &last, blockDim.x, [&](int, double tot) {
+            *out = tot;
+            if (ps.on && ps.seq_alpha) peer_publish1(ps.pd, PEER_CH_ALPHA, ps.seq_alpha, tot);
+        });
     }
 }
 
