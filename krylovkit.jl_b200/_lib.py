@@ -161,7 +161,6 @@ _PROTOS = {
     "b2k_debug_pencil_path": (C.c_int32, []),
     "b2k_debug_set_chain": (C.c_int32, [C.c_int32]),
     "b2k_debug_used_columns": (C.c_int32, [c_ctx, C.c_int32]),
-    "b2k_debug_set_chain_mode": (C.c_int32, [C.c_int32]),
     "b2k_debug_set_onepass_variant": (C.c_int32, [C.c_int32]),
     "b2k_debug_onepass_launch": (C.c_int32, [P(C.c_int32)]),
     "b2k_debug_trace": (C.c_int32, [c_ctx, C.c_int32]),

@@ -70,19 +70,6 @@ __device__ __forceinline__ void peer_boundary(const FusedParams<T>& fp, int i, u
     boundary_sync(ra);
     const PeerDev& pd = fp.ps.pd;
     const int tid = threadIdx.x;
-    if (fp.ph[i].part_h == nullptr) {
-        // boundary in front of a scale phase: the quantity to sum over the ranks is ||w||^2 (channel 2)
-        const unsigned long long sq = fp.ps.seq_norm;
-        if (*flag && tid < 32) {
-            __threadfence();
-            double a = (tid < 16) ? partial_lane_sum(fp.ph[i].part_n, gridDim.x, 1, tid, 16) : 0.0;
-            for (int o = 8; o > 0; o >>= 1) a += __shfl_xor_sync(0xffffffffu, a, o);
-            if (tid == 0) peer_publish1(pd, PEER_CH_NORM, sq, a);
-        }
-        peer_wait(pd, PEER_CH_NORM, sq, tid);
-        boundary_sync(ra);
-        return;
-    }
     const unsigned long long seq = fp.ps.seq_coef[i];
     if (*flag && tid < NCONS) {
         __threadfence();
@@ -178,7 +165,7 @@ k_finalize(const double* __restrict__ A, const double* __restrict__ B, const dou
     FinalizeParams f;
     f.A = A; f.B = B; f.N = N; f.G = G; f.stride = stride; f.k = k; f.res = res; f.off = off; f.noff = noff;
     f.rec = nullptr; f.alpha_col = -1; f.tol = 0.0; f.stop = nullptr; f.ticket = nullptr; f.enabled = 1;
-    f.peer = 0; f.G_local = G; f.norm_done = 0;
+    f.peer = 0; f.G_local = G;
     finalize_block(f, threadIdx.x, sh);
 }
 
@@ -1085,8 +1072,6 @@ int grid_for_rows(const b2k_ctx* ctx, int64_t n) {
     return (int)std::min<int64_t>(ntiles, ctx->num_sms);
 }
 
-bool g_coop_launch = true;   // B2K_COOP_LAUNCH=0: plain launch of the fused sweep (measurement only: no co-residency guarantee)
-
 // Does phase `st` store into a vector that phase `rd` streams (its x or one of its panel columns)?
 template <typename T>
 bool stores_into_stream(const PhaseParams<T>& st, const PhaseParams<T>& rd, const ColList& cl) {
@@ -1115,11 +1100,8 @@ int32_t launch_fused(b2k_ctx* ctx, FusedParams<T>& fp, const ColList& cl, int gr
     fp.barrier_base = ctx->barrier_base;
     ctx->barrier_base += (unsigned)(fp.nph - 1) * (unsigned)grid;
     void* args[] = {(void*)&fp, (void*)&cl};
-    if (g_coop_launch)
-        B2K_CUDA(ctx, cudaLaunchCooperativeKernel((const void*)k_gs_fused<T>, dim3(grid), dim3(NTHREADS),
-                                                  args, SMEM_BYTES, ctx->stream));
-    else    // A/B switch: grid <= #SMs and one CTA per SM by shared memory, i.e. co-resident on an idle device
-        k_gs_fused<T><<<grid, NTHREADS, SMEM_BYTES, ctx->stream>>>(fp, cl);
+    B2K_CUDA(ctx, cudaLaunchCooperativeKernel((const void*)k_gs_fused<T>, dim3(grid), dim3(NTHREADS),
+                                              args, SMEM_BYTES, ctx->stream));
     B2K_LAUNCH_CHECK(ctx);
     return B2K_OK;
 }
@@ -1133,14 +1115,6 @@ int32_t enqueue_finalize(b2k_ctx* ctx, const double* A, const double* B, const d
 }
 
 bool g_l2_hints = true;      // B2K_L2_HINTS=0 switches the eviction-priority hints off (A/B measurements)
-// How a chained step gets its normalised vector v = r/beta:
-//   0 (default): normalisation fused into the SpMV's gather, v written to a column of its own (r's column is
-//      recycled); with the L2 eviction hints r is still partly L2-resident when the SpMV gathers it;
-//   1: a third "scale" phase of the Gram-Schmidt launch normalises w in place — the layout of the reference
-//      (lanczos.jl:257: the residual's storage becomes the basis vector); the extra phase costs the sweep more
-//      than the SpMV saves.
-// B2K_CHAIN_MODE selects; both are bit-identical to stepping.
-int g_chain_mode = 0;
 
 struct Panel {
     void* base;      // space base pointer
@@ -1191,6 +1165,31 @@ PhaseParams<T> base_params(const Panel& pn, int k, const void* x, void* xout) {
     p.alphac = (T)1;
     p.l2_hints = g_l2_hints ? 1 : 0;
     return p;
+}
+
+// The two sweeps of a CGS2 Lanczos step (lanczos.jl:313-324) over the column list of lanczos_cols, as fp.ph[0..1]:
+//   A (project): with `prologue`, w' = (w + c1 v_prev) + c2 v; h = V^T w' -> per-CTA partials (part set 0);
+//   C (update):  the same prologue; w'' = w' - V h stored in place; ||w''||^2 -> per-CTA partials (part set 2).
+// C sums h from A's per-CTA partials; a caller that reduces h elsewhere points C's coefficients there.  The prologue
+// reads c1 / c2 from the device when c1_dev / c2_dev are given (PhaseParams).
+template <typename T>
+void lanczos_sweeps(b2k_ctx* ctx, FusedParams<T>& fp, const Panel& pn, int K1, const VecRef& w, int grid,
+                    bool prologue, double c1, double c2, const double* c1_dev, const double* c2_dev) {
+    memset(&fp, 0, sizeof(fp));
+    PhaseParams<T>& a = fp.ph[0];
+    PhaseParams<T>& c = fp.ph[1];
+    a = base_params<T>(pn, K1, w.ptr, nullptr);
+    c = base_params<T>(pn, K1, w.ptr, w.ptr);
+    if (prologue) {
+        for (PhaseParams<T>* q : {&a, &c}) {
+            q->prologue = 1; q->c1 = (T)c1; q->c2 = (T)c2;
+            q->c1_dev = c1_dev; q->c2_dev = c2_dev;
+        }
+    }
+    a.part_h = b2k_part_set(ctx, 0);
+    c.store_x = 1; c.coef = a.part_h; c.coef_sets = grid; c.coef_stride = B2K_KSTRIDE;
+    c.alphac = (T)-1; c.part_n = b2k_part_set(ctx, 2);
+    fp.kind[0] = 0; fp.kind[1] = 2; fp.nph = 2;
 }
 
 // ------------------------------------------------------------------------------------
@@ -1385,6 +1384,39 @@ int32_t mgs_sweep(b2k_ctx* ctx, const Panel& pn, const VecRef& v, int k, int res
     return B2K_OK;
 }
 
+// One classical pass of a synchronous CGS2 / CGSIR Lanczos step, K1 <= kcap<T>(): d_res[s_h..+K1) = h,
+// d_res[s_n] = ||w||^2.  fused: both sweeps in one cooperative launch (per-phase launches under
+// b2k_debug_set_coop(0)).  Otherwise (row-sharded, or more chunks than ring slots) one launch per sweep, and the
+// all-reduce of the coefficients sits where the grid barrier was.
+template <typename T>
+int32_t lanczos_step_gs(b2k_ctx* ctx, const Panel& pn, int K1, const VecRef& rw, bool prologue, double c1,
+                        double c2, const double* c2_dev, bool fused, int s_h, int s_n) {
+    const int grid = grid_for_rows<T>(ctx, pn.n);
+    ColList cl;
+    lanczos_cols(cl, pn, K1, prologue);
+    FusedParams<T> fp;
+    lanczos_sweeps<T>(ctx, fp, pn, K1, rw, grid, prologue, c1, c2, nullptr, c2_dev);
+    double* PA = fp.ph[0].part_h;
+    double* PN = fp.ph[1].part_n;
+    const int pr = b2k_prof_begin(ctx, 1, (2.0 * K1 + 3.0) * sizeof(T) * (double)pn.n);
+    if (fused && g_use_coop) {
+        B2K_TRY(launch_fused<T>(ctx, fp, cl, grid));
+    } else {
+        B2K_TRY(launch_phase<T>(ctx, fp.ph[0], cl, 0, grid));
+        if (!fused) {
+            B2K_TRY(enqueue_finalize(ctx, PA, nullptr, nullptr, grid, K1, s_h, s_n));
+            B2K_TRY(b2k_allreduce(ctx, ctx->d_res + s_h, K1, pn.sharded));
+            fp.ph[1].coef = ctx->d_res + s_h; fp.ph[1].coef_sets = 1; fp.ph[1].coef_stride = 0;
+        }
+        B2K_TRY(launch_phase<T>(ctx, fp.ph[1], cl, 2, grid));
+    }
+    b2k_prof_end(ctx, pr);
+    if (fused) return enqueue_finalize(ctx, PA, nullptr, PN, grid, K1, s_h, s_n);
+    k_finalize<<<1, NCONS, 0, ctx->stream>>>(PN, nullptr, PN, grid, B2K_KSTRIDE, 0, ctx->d_res, 0, s_n);
+    B2K_LAUNCH_CHECK(ctx);
+    return b2k_allreduce(ctx, ctx->d_res + s_n, 1, pn.sharded);
+}
+
 }  // namespace
 
 int32_t b2k_cross_init(b2k_ctx* ctx);     // b2k_basis_cross_inner, below
@@ -1392,8 +1424,6 @@ int32_t b2k_cross_init(b2k_ctx* ctx);     // b2k_basis_cross_inner, below
 // called once per context (ctx.cu): opt in to > 48 KB dynamic shared memory
 int32_t b2k_basis_init(b2k_ctx* ctx) {
     if (const char* e = getenv("B2K_L2_HINTS")) g_l2_hints = e[0] != '0';
-    if (const char* e = getenv("B2K_CHAIN_MODE")) g_chain_mode = e[0] == '1' ? 1 : 0;
-    if (const char* e = getenv("B2K_COOP_LAUNCH")) g_coop_launch = e[0] != '0';
     if (const char* e = getenv("B2K_TRANSFORM_UR")) g_transform_ur = (e[0] >= '0' && e[0] <= '3') ? e[0] - '0' : 0;
     if (const char* e = getenv("B2K_TRANSFORM_HYB")) g_transform_hyb = (e[0] >= '0' && e[0] <= '3') ? e[0] - '0' : 0;
 #define SETATTR(fn, bytes) \
@@ -1689,74 +1719,14 @@ extern "C" int32_t b2k_lanczos_expand(b2k_ctx* ctx, const b2k_op* op, const b2k_
                 nold = beta;
                 continue;
             }
-            if (fusable) {
-                const int grid = f64 ? grid_for_rows<double>(ctx, pn.n) : grid_for_rows<float>(ctx, pn.n);
-                ColList cl;
-                lanczos_cols(cl, pn, K1, prologue);
-                double* PA = b2k_part_set(ctx, 0);
-                double* PN = b2k_part_set(ctx, 2);
-#define BUILD_AND_LAUNCH(T)                                                                   \
-    {                                                                                         \
-        FusedParams<T> fp;                                                                    \
-        memset(&fp, 0, sizeof(fp));                                                           \
-        PhaseParams<T> a = base_params<T>(pn, K1, rw.ptr, nullptr);                           \
-        PhaseParams<T> c = base_params<T>(pn, K1, rw.ptr, rw.ptr);                            \
-        if (prologue) {                                                                       \
-            for (PhaseParams<T>* q : {&a, &c}) {                                              \
-                q->prologue = 1; q->c1 = (T)(-beta_old); q->c2 = (T)(-alpha);                 \
-                if (defer_alpha) q->c2_dev = ctx->d_res + S_A0;                               \
-            }                                                                                 \
-        }                                                                                     \
-        a.part_h = PA;                                                                        \
-        c.store_x = 1; c.coef = PA; c.coef_sets = grid; c.coef_stride = B2K_KSTRIDE;          \
-        c.alphac = (T)-1; c.part_n = PN;                                                      \
-        fp.ph[0] = a; fp.kind[0] = 0; fp.ph[1] = c; fp.kind[1] = 2; fp.nph = 2;               \
-        const int pr = b2k_prof_begin(ctx, 1, (2.0 * K1 + 3.0) * sizeof(T) * (double)pn.n);   \
-        if (g_use_coop) { B2K_TRY(launch_fused<T>(ctx, fp, cl, grid)); }                      \
-        else {                                                                                \
-            B2K_TRY(launch_phase<T>(ctx, fp.ph[0], cl, 0, grid));                             \
-            B2K_TRY(launch_phase<T>(ctx, fp.ph[1], cl, 2, grid));                             \
-        }                                                                                     \
-        b2k_prof_end(ctx, pr);                                                                \
-    }
-                if (f64) BUILD_AND_LAUNCH(double) else BUILD_AND_LAUNCH(float)
-#undef BUILD_AND_LAUNCH
-                B2K_TRY(enqueue_finalize(ctx, PA, nullptr, PN, grid, K1, S_H, S_N));
-                B2K_TRY(b2k_fetch_results(ctx, S_A0 + 1, 0));
-                if (defer_alpha) alpha = ctx->h_res[S_A0];
-            } else if (one_pass) {
-                // row-sharded (or > resident-tile) variant of the same two sweeps: one launch per
-                // sweep, the all-reduce of the coefficients sits where the grid barrier was
-                const int grid = f64 ? grid_for_rows<double>(ctx, pn.n) : grid_for_rows<float>(ctx, pn.n);
-                ColList cl;
-                lanczos_cols(cl, pn, K1, prologue);
-                double* PA = b2k_part_set(ctx, 0);
-                double* PN = b2k_part_set(ctx, 2);
-#define SPLIT_SWEEPS(T)                                                                       \
-    {                                                                                         \
-        PhaseParams<T> a = base_params<T>(pn, K1, rw.ptr, nullptr);                           \
-        PhaseParams<T> c = base_params<T>(pn, K1, rw.ptr, rw.ptr);                            \
-        if (prologue) {                                                                       \
-            for (PhaseParams<T>* q : {&a, &c}) {                                              \
-                q->prologue = 1; q->c1 = (T)(-beta_old); q->c2 = (T)(-alpha);                 \
-                if (defer_alpha) q->c2_dev = ctx->d_res + S_A0;                               \
-            }                                                                                 \
-        }                                                                                     \
-        a.part_h = PA;                                                                        \
-        const int pr = b2k_prof_begin(ctx, 1, (2.0 * K1 + 3.0) * sizeof(T) * (double)pn.n);   \
-        B2K_TRY(launch_phase<T>(ctx, a, cl, 0, grid));                                        \
-        B2K_TRY(enqueue_finalize(ctx, PA, nullptr, nullptr, grid, K1, S_H, S_N));             \
-        B2K_TRY(b2k_allreduce(ctx, ctx->d_res + S_H, K1, pn.sharded));                        \
-        c.store_x = 1; c.coef = ctx->d_res + S_H; c.coef_sets = 1; c.coef_stride = 0;         \
-        c.alphac = (T)-1; c.part_n = PN;                                                      \
-        B2K_TRY(launch_phase<T>(ctx, c, cl, 2, grid));                                        \
-        b2k_prof_end(ctx, pr);                                                                \
-    }
-                if (f64) SPLIT_SWEEPS(double) else SPLIT_SWEEPS(float)
-#undef SPLIT_SWEEPS
-                k_finalize<<<1, NCONS, 0, ctx->stream>>>(PN, nullptr, PN, grid, B2K_KSTRIDE, 0, ctx->d_res, 0, S_N);
-                B2K_LAUNCH_CHECK(ctx);
-                B2K_TRY(b2k_allreduce(ctx, ctx->d_res + S_N, 1, pn.sharded));
+            if (one_pass) {
+                const double* c2_dev = defer_alpha ? ctx->d_res + S_A0 : nullptr;
+                if (f64)
+                    B2K_TRY(lanczos_step_gs<double>(ctx, pn, K1, rw, prologue, -beta_old, -alpha, c2_dev, fusable,
+                                                    S_H, S_N));
+                else
+                    B2K_TRY(lanczos_step_gs<float>(ctx, pn, K1, rw, prologue, -beta_old, -alpha, c2_dev, fusable,
+                                                   S_H, S_N));
                 B2K_TRY(b2k_fetch_results(ctx, S_A0 + 1, 0));
                 if (defer_alpha) alpha = ctx->h_res[S_A0];
             } else {
@@ -1873,34 +1843,16 @@ bool chain_ok(const b2k_ctx* ctx, const b2k_op* op, const b2k_vec* cols, int32_t
 }
 
 template <typename T>
-int32_t chain_step_gs(b2k_ctx* ctx, const Panel& pn, int K1, const VecRef& rw, const VecRef& vprev,
-                      const VecRef& rv, double* rec_prev, double* rec, double tol, const PeerStep* psp,
-                      bool scale_after) {
+int32_t chain_step_gs(b2k_ctx* ctx, const Panel& pn, int K1, const VecRef& rw, double* rec_prev, double* rec,
+                      double tol, const PeerStep* psp) {
     const int grid = grid_for_rows<T>(ctx, pn.n);
     ColList cl;
     lanczos_cols(cl, pn, K1, true);
     double* PA = b2k_part_set(ctx, 0);
     double* PN = b2k_part_set(ctx, 2);
     FusedParams<T> fp;
-    memset(&fp, 0, sizeof(fp));
-    PhaseParams<T> a = base_params<T>(pn, K1, rw.ptr, nullptr);
-    PhaseParams<T> c = base_params<T>(pn, K1, rw.ptr, rw.ptr);
-    for (PhaseParams<T>* q : {&a, &c}) {
-        q->prologue = 1;
-        q->c1_dev = rec_prev + 2;     // beta of the previous step
-        q->c2_dev = rec + 0;          // <v, A v> of this step
-    }
-    a.part_h = PA;
-    c.store_x = 1; c.coef = PA; c.coef_sets = grid; c.coef_stride = B2K_KSTRIDE;
-    c.alphac = (T)-1; c.part_n = PN;
-    fp.ph[0] = a; fp.kind[0] = 0; fp.ph[1] = c; fp.kind[1] = 2; fp.nph = 2;
-    if (scale_after) {
-        // third phase: w <- w / beta in place while its tiles are hot in L2 — the next step's v (lanczos.jl:257)
-        PhaseParams<T> sc = base_params<T>(pn, 0, rw.ptr, rw.ptr);
-        sc.store_x = 1; sc.beta_mode = 2; sc.scale_mode = 1;
-        sc.scale_norm = PN; sc.scale_G = grid; sc.scale_stride = 1; sc.scale_tol = tol;
-        fp.ph[2] = sc; fp.kind[2] = 2; fp.nph = 3;
-    }
+    // the prologue's beta is the previous step's, <v, A v> this step's (the SpMV wrote it)
+    lanczos_sweeps<T>(ctx, fp, pn, K1, rw, grid, true, 0.0, 0.0, rec_prev + 2, rec + 0);
     fp.stop = reinterpret_cast<const int*>(ctx->d_sync + B2K_SYNC_STOP);
     fp.trace = ctx->d_trace;
     fp.fin.A = PA; fp.fin.B = nullptr; fp.fin.N = PN; fp.fin.G = grid; fp.fin.stride = B2K_KSTRIDE;
@@ -1908,7 +1860,7 @@ int32_t chain_step_gs(b2k_ctx* ctx, const Panel& pn, int K1, const VecRef& rw, c
     fp.fin.alpha_col = K1 - 1; fp.fin.tol = tol;
     fp.fin.stop = reinterpret_cast<int*>(ctx->d_sync + B2K_SYNC_STOP);
     fp.fin.ticket = ctx->d_sync + B2K_SYNC_GSFIN; fp.fin.enabled = 1;
-    fp.fin.peer = 0; fp.fin.G_local = grid; fp.fin.norm_done = 0;
+    fp.fin.peer = 0; fp.fin.G_local = grid;
     if (psp && psp->on) {
         const PeerStep& ps = *psp;
         fp.ps = ps;
@@ -1927,19 +1879,13 @@ int32_t chain_step_gs(b2k_ctx* ctx, const Panel& pn, int K1, const VecRef& rw, c
         fp.ph[1].coef_sets = ps.pd.nranks;
         fp.ph[1].coef_stride = PEER_SLOT;
         fp.fin.A = fp.ph[1].coef; fp.fin.G = ps.pd.nranks; fp.fin.stride = PEER_SLOT; fp.fin.peer = 1;
-        const int last = fp.nph - 1;      // the phase that stores the vector the next SpMV reads
-        if (scale_after) {
-            fp.ph[2].scale_norm = slot(PEER_CH_NORM, ps.seq_norm);
-            fp.ph[2].scale_G = ps.pd.nranks;
-            fp.ph[2].scale_stride = PEER_SLOT;
-            fp.fin.norm_done = 1;         // exchanged at the boundary in front of the scale phase
-        }
         // rows the neighbours need for their next SpMV leave with the final store
         if (ps.seq_halo) {
-            fp.ph[last].send_lo = ps.send_lo;
-            fp.ph[last].send_hi = ps.send_hi;
-            fp.ph[last].halo_dn = ps.send_lo ? reinterpret_cast<T*>(ps.pd.win[ps.pd.rank - 1] + ps.dn_off) : nullptr;
-            fp.ph[last].halo_up = ps.send_hi ? reinterpret_cast<T*>(ps.pd.win[ps.pd.rank + 1] + ps.up_off) : nullptr;
+            PhaseParams<T>& c = fp.ph[1];
+            c.send_lo = ps.send_lo;
+            c.send_hi = ps.send_hi;
+            c.halo_dn = ps.send_lo ? reinterpret_cast<T*>(ps.pd.win[ps.pd.rank - 1] + ps.dn_off) : nullptr;
+            c.halo_up = ps.send_hi ? reinterpret_cast<T*>(ps.pd.win[ps.pd.rank + 1] + ps.up_off) : nullptr;
         }
     }
     const int pr = b2k_prof_begin(ctx, 1, (2.0 * K1 + 3.0) * sizeof(T) * (double)pn.n);
@@ -1961,22 +1907,18 @@ int32_t lanczos_chain(b2k_ctx* ctx, const b2k_op* op, b2k_vec* cols, int32_t k, 
     }
     k_lanczos_seed<<<1, 1, 0, ctx->stream>>>(rec0, beta_old, d_stop);
     B2K_LAUNCH_CHECK(ctx);
-    const bool inplace = g_chain_mode == 1;
     std::vector<b2k_vec> touched, Vh, Wh;
     touched.push_back(cols[k]);
     int32_t enq = 0, rc = B2K_OK;
     const bool dist = ctx->nranks > 1;
     unsigned long long halo_seq = 0;
-    if (inplace) B2K_TRY(b2k_vec_scale(ctx, cols[k], cols[k], 1.0 / beta_old));   // v = r/beta of the first step
     for (int32_t i = 0; i < nsteps; ++i) {
         const int32_t K = k + i;                 // basis size before this step's push!
         const b2k_vec R = cols[K];
-        b2k_vec V = R, W = -1;
-        if (!inplace) {
-            rc = b2k_vec_alloc(ctx, space, &V);
-            if (rc != B2K_OK) break;
-            touched.push_back(V);
-        }
+        b2k_vec V = -1, W = -1;
+        rc = b2k_vec_alloc(ctx, space, &V);
+        if (rc != B2K_OK) break;
+        touched.push_back(V);
         rc = b2k_vec_alloc(ctx, space, &W);
         if (rc != B2K_OK) break;
         touched.push_back(W);
@@ -1988,13 +1930,10 @@ int32_t lanczos_chain(b2k_ctx* ctx, const b2k_op* op, b2k_vec* cols, int32_t k, 
         if (rc != B2K_OK) break;
         double* rec_prev = rec0 + (size_t)B2K_REC * i;
         double* rec = rec0 + (size_t)B2K_REC * (i + 1);
-        const bool scale_after = inplace && (i + 1 < nsteps);   // the batch's last residual stays unnormalised
         SpmvFuse fz;
         memset(&fz, 0, sizeof(fz));
-        if (!inplace) {
-            fz.xscale = rec_prev + 3;
-            fz.vout = rV.ptr;
-        }
+        fz.xscale = rec_prev + 3;
+        fz.vout = rV.ptr;
         fz.stop = d_stop;
         fz.dot_self = 1;
         fz.l2_hints = g_l2_hints ? 1 : 0;
@@ -2013,12 +1952,9 @@ int32_t lanczos_chain(b2k_ctx* ctx, const b2k_op* op, b2k_vec* cols, int32_t k, 
             ps.seq_norm = b2k_peer_next_seq(ctx, PEER_CH_NORM);
             fz.seq_alpha = ps.seq_alpha;
             fz.seq_halo = halo_seq;                    // 0: the apply pushes its operand's boundary rows itself
-            halo_seq = 0;
-            if (!inplace || scale_after) {             // this step's Gram-Schmidt launch pushes the next operand's
-                halo_seq = b2k_peer_next_seq(ctx, 4);
-                rc = b2k_op_peer_halo(ctx, op, halo_seq, &ps);
-                if (rc != B2K_OK) break;
-            }
+            halo_seq = b2k_peer_next_seq(ctx, 4);      // this step's Gram-Schmidt launch pushes the next operand's
+            rc = b2k_op_peer_halo(ctx, op, halo_seq, &ps);
+            if (rc != B2K_OK) break;
         }
         rc = b2k_enqueue_apply_fused(ctx, op, rR, rW, 0.0, 1.0, false, nullptr, rec + 0, &fz);
         if (rc != B2K_OK) break;
@@ -2026,14 +1962,14 @@ int32_t lanczos_chain(b2k_ctx* ctx, const b2k_op* op, b2k_vec* cols, int32_t k, 
         Panel pn;
         rc = make_panel(ctx, cols, K + 1, &pn);
         if (rc != B2K_OK) break;
-        rc = f64 ? chain_step_gs<double>(ctx, pn, K + 1, rW, vprev, rV, rec_prev, rec, tol, &ps, scale_after)
-                 : chain_step_gs<float>(ctx, pn, K + 1, rW, vprev, rV, rec_prev, rec, tol, &ps, scale_after);
+        rc = f64 ? chain_step_gs<double>(ctx, pn, K + 1, rW, rec_prev, rec, tol, &ps)
+                 : chain_step_gs<float>(ctx, pn, K + 1, rW, rec_prev, rec, tol, &ps);
         if (rc != B2K_OK) break;
         cols[K + 1] = W;                         // ... and w the new residual
         Vh.push_back(V);
         Wh.push_back(W);
-        // mode 0: r's column has been consumed; later steps may reuse it (stream order keeps that safe)
-        if (!inplace) ctx->spaces[space].used[B2K_VEC_COL(R)] = 0;
+        // r's column has been consumed; later steps may reuse it (stream order keeps that safe)
+        ctx->spaces[space].used[B2K_VEC_COL(R)] = 0;
         ++enq;
     }
     int32_t d = 0;
@@ -2063,11 +1999,6 @@ int32_t lanczos_chain(b2k_ctx* ctx, const b2k_op* op, b2k_vec* cols, int32_t k, 
     } else {
         sp.used[B2K_VEC_COL(touched[0])] = 1;    // nothing ran: r is still r
         cols[k] = touched[0];
-        if (inplace) {
-            // the residual was normalised for a first step that could not be enqueued: undo (an error path —
-            // slab exhausted — where the caller gets its r back to rounding)
-            b2k_vec_scale(ctx, cols[k], cols[k], beta_old);
-        }
     }
     *steps_done = d;
     *r_out = cols[k + d];
@@ -2076,11 +2007,6 @@ int32_t lanczos_chain(b2k_ctx* ctx, const b2k_op* op, b2k_vec* cols, int32_t k, 
 
 extern "C" int32_t b2k_debug_set_chain(int32_t on) {
     g_use_chain = on != 0;
-    return B2K_OK;
-}
-
-extern "C" int32_t b2k_debug_set_chain_mode(int32_t mode) {
-    g_chain_mode = mode == 0 ? 0 : 1;
     return B2K_OK;
 }
 

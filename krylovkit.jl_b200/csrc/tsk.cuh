@@ -94,14 +94,6 @@ struct PhaseParams {
     T* halo_dn;
     T* halo_up;
     int64_t send_lo, send_hi;
-    // scale phase (UPDATE with k == 0): x'' = x / beta with beta = sqrt(||x||^2) taken from the previous phase's
-    // norm partials (single GPU: G per-CTA partials; row-sharded: the nranks partials in my peer window) — the
-    // normalisation v = r/beta of lanczos.jl:257 done while the tiles of w are still hot in L2.  beta <= scale_tol
-    // (breakdown): nothing is stored, the vector stays the unnormalised residual.
-    int32_t scale_mode;
-    const double* scale_norm;
-    int32_t scale_G, scale_stride;
-    double scale_tol;
     int32_t store_x; // write x'' (UPDATE) to xout
     int32_t l2_hints; // panel loads evict_first, the stored vector evict_last (common.cuh)
     // UPDATE: x'' = betax*x' + sum_j Q[:,j]*cs[j],  cs[j] = alphac * sum_g coef[g*stride+j]
@@ -314,27 +306,6 @@ __device__ __forceinline__ void consumer_phase(const PhaseParams<T>& p, const Sm
     T nrm = (T)0;
     int buf = 0;
     const uint64_t pol_last = p.l2_hints ? l2_policy_evict_last() : 0;
-    T betax = p.betax;
-    bool do_store = p.store_x != 0;
-    if (UPDATE && p.scale_mode) {
-        double* shn = reinterpret_cast<double*>(sm.raw + OFF_RED + 128);
-        if (tid < 32) {
-            double a;
-            if (p.scale_stride == 1) {      // per-CTA partials: the lanes and order of finalize_block
-                a = (tid < 16) ? partial_lane_sum(p.scale_norm, p.scale_G, 1, tid, 16) : 0.0;
-                for (int o = 8; o > 0; o >>= 1) a += __shfl_xor_sync(0xffffffffu, a, o);
-            } else {                        // per-rank partials in the peer window: rank order (peer_sum1)
-                a = 0.0;
-                for (int g = 0; g < p.scale_G; ++g)
-                    a += *reinterpret_cast<const volatile double*>(p.scale_norm + (size_t)g * p.scale_stride);
-            }
-            if (tid == 0) shn[0] = a;
-        }
-        named_bar_sync(1, NCONS);
-        const double beta = sqrt(shn[0]);
-        if (beta <= p.scale_tol) do_store = false;
-        betax = (T)(1.0 / beta);
-    }
     T c1 = p.c1, c2 = p.c2;
     if (p.c1_dev) c1 = (T)(-(*reinterpret_cast<const volatile double*>(p.c1_dev)));
     if (p.c2_dev) {
@@ -365,7 +336,7 @@ __device__ __forceinline__ void consumer_phase(const PhaseParams<T>& p, const Sm
         T acc = xv;
         const uint32_t s0 = st.s, ph0 = st.ph;
         if (UPDATE) {
-            acc = (p.beta_mode == 0) ? (T)0 : (p.beta_mode == 1 ? xv : betax * xv);
+            acc = (p.beta_mode == 0) ? (T)0 : (p.beta_mode == 1 ? xv : p.betax * xv);
             for (int c = 0; c < nch; ++c) {
                 mbar_wait(sm.full + 8 * st.s, st.ph);
                 const T* slot = reinterpret_cast<const T*>(sm.raw + OFF_RING + st.s * SLOT_BYTES);
@@ -393,7 +364,7 @@ __device__ __forceinline__ void consumer_phase(const PhaseParams<T>& p, const Sm
             }
             if (tid >= rt) acc = (T)0;
         }
-        if (do_store && tid < rt) {
+        if (p.store_x && tid < rt) {
             if (p.l2_hints) st_hint(p.xout + r0 + tid, acc, pol_last);
             else p.xout[r0 + tid] = acc;
             if (UPDATE && !PROJECT) {
@@ -502,7 +473,6 @@ struct FinalizeParams {
     // N the LOCAL per-CTA norm partials (G_local of them); the norm and <v, A v> are summed over ranks here
     int peer;
     int G_local;
-    int norm_done;      // row-sharded: ||w||^2 was already exchanged at a phase boundary (scale phase): just read it
 };
 
 // `sh` : >= 2 doubles of shared memory; `barrier_id` : named barrier the NCONS calling threads may use
@@ -530,10 +500,8 @@ __device__ __forceinline__ void finalize_block(const FinalizeParams& f, int tid,
     double alpha0 = f.rec ? f.rec[0] : 0.0;
     if (f.peer && ps) {
         // ||w||^2: publish my partial to every rank, wait for theirs in my window, add in rank order
-        if (!f.norm_done) {
-            if (tid == 0) peer_publish1(ps->pd, PEER_CH_NORM, ps->seq_norm, n2);
-            peer_wait(ps->pd, PEER_CH_NORM, ps->seq_norm, tid);
-        }
+        if (tid == 0) peer_publish1(ps->pd, PEER_CH_NORM, ps->seq_norm, n2);
+        peer_wait(ps->pd, PEER_CH_NORM, ps->seq_norm, tid);
         named_bar_sync(1, NCONS);
         if (tid == 0) {
             n2 = peer_sum1(ps->pd, PEER_CH_NORM, ps->seq_norm, 0);

@@ -122,14 +122,9 @@ class HostSimLib:
         self.next_id = 1000
         self.err = b""
         self.chain = True          # b2k_lanczos_expand_many follows the device-chained handle contract (CGS2)
-        self.chain_mode = 0        # 0 (library default): v in a column of its own; 1: residual normalised in place
 
     def b2k_debug_used_columns(self, h, space):
         return len(self._c(h).spaces[space].cols)
-
-    def b2k_debug_set_chain_mode(self, mode):
-        self.chain_mode = 0 if mode == 0 else 1
-        return L.OK
 
     def b2k_debug_set_onepass_variant(self, v):
         return L.OK if v in (0, 1) else L.EINVAL            # one numpy product stands for both kernels
@@ -619,7 +614,7 @@ class HostSimLib:
                 self.b2k_vec_free(h, wref.value)
                 return st
             alphas[i], betas[i] = a.value, b.value
-            if self.chain and self.chain_mode == 0 and alg in (L.CGS2, L.MGS2B):
+            if self.chain and alg in (L.CGS2, L.MGS2B):
                 # the device-chained contract: the normalised vector lives in a column of its own and the old
                 # residual's column goes back to the slab (it may be handed out again right away)
                 vref = C.c_int32()

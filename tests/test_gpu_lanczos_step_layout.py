@@ -4,9 +4,10 @@ The sweeps of a CGS2 Lanczos step list the basis columns rotated by two, [v_prev
 w' = (w - beta v_prev) - alpha v per row from the first chunk of each tile in both sweeps (w' is never stored), and
 let the producer warps run through the phase boundary.  The column widths below put the rotated chunk boundaries on
 every side of v_prev and v (8 columns a chunk in Float64, 16 in Float32, up to a full 12-chunk ring), at row counts
-with a ragged last tile, with fewer row tiles than SMs and with CTAs that own two tiles.
+with a ragged last tile, with fewer row tiles than SMs and with CTAs that own two tiles (the chained batch also with
+full tiles only and with CTAs that own four).
 
-1. A device-chained batch (both chain layouts) equals the loop of synchronous steps bit for bit.
+1. A device-chained batch equals the loop of synchronous steps bit for bit.
 2. One synchronous step (fused sweep, split sweeps, and the launch per phase) equals the same step recomputed from
    primitives that stream one vector through the original column order: vec_axpy2 for the prologue, basis_project and
    basis_unproject for the pass.  Not to the bit: the primitives take <v, A v> and the coefficients from other
@@ -35,17 +36,20 @@ f64, f32 = np.float64, np.float32
 # so with 132 SMs some CTAs own two tiles
 SIZES = [(97, 61), (211, 173)]
 SIZE_IDS = ["n5917", "n36503"]
+# the chained batch also at 8192 rows = 32 full tiles (no ragged tile) and 105463 rows = 411 full tiles + 247 rows, so
+# with 132 SMs the CTA that owns the ragged tile owns four
+CHAIN_SIZES = SIZES + [(128, 64), (401, 263)]
+CHAIN_SIZE_IDS = SIZE_IDS + ["n8192", "n105463"]
 
 
 def unit(dtype):
     return 2.0 ** -53 if dtype == f64 else 2.0 ** -24
 
 
-def run_batch(chain_mode, dtype, nsteps, nx, ny):
-    """initialize + one b2k_lanczos_expand_many batch from k = 1; chain_mode None = the loop of synchronous steps"""
+def run_batch(chain, dtype, nsteps, nx, ny):
+    """initialize + one b2k_lanczos_expand_many batch from k = 1; chain False = the loop of synchronous steps"""
     lib = L.load()
-    lib.b2k_debug_set_chain(0 if chain_mode is None else 1)
-    lib.b2k_debug_set_chain_mode(chain_mode or 0)
+    lib.b2k_debug_set_chain(1 if chain else 0)
     try:
         n = nx * ny
         ctx = kk.B200Context(n, nsteps + 8, dtype=dtype)
@@ -64,18 +68,16 @@ def run_batch(chain_mode, dtype, nsteps, nx, ny):
         return out
     finally:
         lib.b2k_debug_set_chain(1)
-        lib.b2k_debug_set_chain_mode(0)
 
 
-@pytest.mark.parametrize("nx,ny", SIZES, ids=SIZE_IDS)
-@pytest.mark.parametrize("chain_mode", [0, 1], ids=["vout", "inplace"])
+@pytest.mark.parametrize("nx,ny", CHAIN_SIZES, ids=CHAIN_SIZE_IDS)
 @pytest.mark.parametrize("dtype,K1max", [(f64, 96), (f32, 192)], ids=["float64", "float32"])
-def test_chained_batch_equals_stepping(dtype, K1max, chain_mode, nx, ny):
+def test_chained_batch_equals_stepping(dtype, K1max, nx, ny):
     """A batch from k = 1 to K1 = K1max runs one chained step at every K1 in 2..K1max (among them 2, 3, 8, 9, 10, 16,
     17, 60, 95, 96 in Float64 and 2, 16, 17, 18, 192 in Float32): alpha, beta, V and r equal the stepping loop's."""
     nsteps = K1max - 1
-    a1, b1, V1, r1, nl1 = run_batch(chain_mode, dtype, nsteps, nx, ny)
-    a0, b0, V0, r0, nl0 = run_batch(None, dtype, nsteps, nx, ny)
+    a1, b1, V1, r1, nl1 = run_batch(True, dtype, nsteps, nx, ny)
+    a0, b0, V0, r0, nl0 = run_batch(False, dtype, nsteps, nx, ny)
     assert nl1 <= 2 * nsteps + 2 and nl0 >= 3 * nsteps, (nl1, nl0)     # the batch was chained, the loop was not
     assert np.array_equal(a1, a0) and np.array_equal(b1, b0)
     assert np.array_equal(V1, V0) and np.array_equal(r1, r0)

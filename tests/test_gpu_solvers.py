@@ -792,10 +792,9 @@ def test_zero_start_vector_raises():
 
 def _expand_many_run(chain, nx=97, ny=61, steps=30, tol=0.0, diag=None, orth=None):
     """initialize + one b2k_lanczos_expand_many batch; returns (alphas, betas, V (host), r (host), free columns).
-    chain: False = one synchronous step at a time; "inplace" (= True) / "vout" = the two device-chained layouts."""
+    chain: False = one synchronous step at a time, True = the device-chained steps."""
     lib = L.load()
     lib.b2k_debug_set_chain(1 if chain else 0)
-    lib.b2k_debug_set_chain_mode(0 if chain == "vout" else 1)
     try:
         n = nx * ny
         ctx = kk.B200Context(n, steps + 8)
@@ -823,15 +822,14 @@ def _expand_many_run(chain, nx=97, ny=61, steps=30, tol=0.0, diag=None, orth=Non
         return out
     finally:
         lib.b2k_debug_set_chain(1)
-        lib.b2k_debug_set_chain_mode(0)
 
 
 def test_chained_lanczos_batch_is_bit_identical_to_stepping():
     """b2k_lanczos_expand_many with the device-chained steps (normalisation fused into the SpMV gather, scalars
     kept in device records, in-kernel finalisation, no host round trip) gives the same bits as one synchronous
     b2k_lanczos_expand per step: same kernels' arithmetic, same operand bits (lanczos.jl:250-272, 313-324)."""
-    for orth, mode in ((kk.cgs2, "inplace"), (kk.cgs2, "vout"), (kk.mgs2b, "inplace"), (kk.mgs2b, "vout")):
-        d1, a1, b1, V1, r1 = _expand_many_run(mode, orth=orth)
+    for orth in (kk.cgs2, kk.mgs2b):
+        d1, a1, b1, V1, r1 = _expand_many_run(True, orth=orth)
         d0, a0, b0, V0, r0 = _expand_many_run(False, orth=orth)
         assert d1 == d0 == 30
         if orth is kk.cgs2:
@@ -852,12 +850,11 @@ def test_chained_lanczos_batch_stops_at_breakdown_on_the_device():
     n = 3000
     d = np.repeat([1.0, 2.5, 7.0, 11.0], n // 4)
     d0, a0, b0, V0, r0 = _expand_many_run(False, nx=n, ny=1, steps=12, tol=1e-9, diag=d)
-    for mode in ("inplace", "vout"):
-        d1, a1, b1, V1, r1 = _expand_many_run(mode, nx=n, ny=1, steps=12, tol=1e-9, diag=d)
-        assert d1 == d0 == 3                    # 4 distinct eigenvalues: the Krylov space is exhausted at K = 4
-        assert np.array_equal(a1, a0) and np.array_equal(b1, b0)
-        assert np.array_equal(V1, V0) and np.array_equal(r1, r0)
-        assert b1[-1] <= 1e-9
+    d1, a1, b1, V1, r1 = _expand_many_run(True, nx=n, ny=1, steps=12, tol=1e-9, diag=d)
+    assert d1 == d0 == 3                    # 4 distinct eigenvalues: the Krylov space is exhausted at K = 4
+    assert np.array_equal(a1, a0) and np.array_equal(b1, b0)
+    assert np.array_equal(V1, V0) and np.array_equal(r1, r0)
+    assert b1[-1] <= 1e-9
 
 
 def test_blocklanczos_fast_block_mode_matches_reference_mode():
