@@ -155,6 +155,12 @@ _PROTOS = {
     "b2k_debug_set_csr_compact": (C.c_int32, [C.c_int32]),
     "b2k_debug_spmv_kernel": (C.c_int32, []),
     "b2k_debug_csr_format": (C.c_int32, [c_op]),
+    "b2k_debug_spmv_launch": (C.c_int32, [P(C.c_int32)]),
+    "b2k_debug_op_tiles": (C.c_int32, [c_ctx, c_op, P(C.c_int32), P(C.c_int32)]),
+    # x, y, a0, a1, shifted, dotv, xscale, vout, dot_self, dot_sub vector and scale, l2_hints, stop, no_slot, dot
+    "b2k_debug_apply_fused": (C.c_int32, [c_ctx, c_op, c_vec, c_vec, C.c_double, C.c_double, C.c_int32, c_vec,
+                                          P(C.c_double), c_vec, C.c_int32, c_vec, C.c_double, C.c_int32, C.c_int32,
+                                          C.c_int32, P(C.c_double)]),
     "b2k_debug_set_dmma": (C.c_int32, [C.c_int32]),
     "b2k_debug_set_transform": (C.c_int32, [C.c_int32]),
     "b2k_debug_transform_kernel": (C.c_int32, []),

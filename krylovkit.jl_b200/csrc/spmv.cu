@@ -2079,6 +2079,10 @@ static bool g_csr_compact = true;
 // the CSR SpMV kernel the last apply launched (b2k_debug_spmv_kernel): 0 = none yet, 1 = k_spmv_stream,
 // 2 = k_spmv_pipe, 3 = k_spmv_compact
 static int g_spmv_kernel = 0;
+// the last single-operator SpMV launch that passed its checks (b2k_debug_spmv_launch): {kernel (1 = k_spmv_stream,
+// 2 = k_spmv_pipe, 3 = k_spmv_compact, 4 = k_stencil_apply), instance, grid, nblk}.  instance: k_spmv_pipe's variant
+// (g_spmv_variant), k_spmv_compact's <VS, IS> as 1 (VS = float) | 2 (IS = int16_t), else 0.
+static int32_t g_spmv_launch[4] = {0, 0, 0, 0};
 
 extern "C" int32_t b2k_debug_set_csr_compact(int32_t on) {
     g_csr_compact = on != 0;
@@ -2092,6 +2096,68 @@ extern "C" int32_t b2k_debug_spmv_kernel(void) { return g_spmv_kernel; }
 extern "C" int32_t b2k_debug_csr_format(const b2k_op* op) {
     if (!op || !op->crp) return 0;
     return 4 | (op->ccol ? 2 : 0) | (op->cvals ? 1 : 0);
+}
+
+extern "C" int32_t b2k_debug_spmv_launch(int32_t* out) {
+    if (!out) return B2K_EINVAL;
+    for (int i = 0; i < 4; ++i) out[i] = g_spmv_launch[i];
+    return B2K_OK;
+}
+
+// The tile boundaries of a CSR operator: *nblk, and rowblk[0 .. nblk] when rowblk is given (nblk = 0 for a matrix-free
+// stencil).
+extern "C" int32_t b2k_debug_op_tiles(b2k_ctx* ctx, const b2k_op* op, int32_t* rowblk, int32_t* nblk) {
+    if (!ctx || !op || !nblk) return B2K_EINVAL;
+    *nblk = op->nblk;
+    if (rowblk && op->rowblk) {
+        B2K_CUDA(ctx, cudaMemcpyAsync(rowblk, op->rowblk, sizeof(int32_t) * (op->nblk + 1), cudaMemcpyDeviceToHost,
+                                      ctx->stream));
+        B2K_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+    }
+    return B2K_OK;
+}
+
+// b2k_enqueue_apply_fused with a SpmvFuse built from host arguments, through the production checks.  Vectors < 0 are
+// absent; xscale (null: none) and dsub_scale are copied to device scratch of their own, and the stop flag is a private
+// device int set to `stop`.  The dot goes to a scratch slot prefilled with *dot (no slot at all when no_slot is set);
+// on return *dot is what the slot holds, so a launch that did not write it returns the value passed in.
+extern "C" int32_t b2k_debug_apply_fused(b2k_ctx* ctx, const b2k_op* op, b2k_vec x, b2k_vec y, double a0, double a1,
+                                         int32_t shifted, b2k_vec dotv, const double* xscale, b2k_vec vout,
+                                         int32_t dot_self, b2k_vec dsub, double dsub_scale, int32_t l2_hints,
+                                         int32_t stop, int32_t no_slot, double* dot) {
+    if (!ctx || !op || !dot) return B2K_EINVAL;
+    VecRef rx, ry, rd, rv, rs;
+    B2K_TRY(b2k_resolve(ctx, x, &rx));
+    B2K_TRY(b2k_resolve(ctx, y, &ry));
+    if (dotv >= 0) B2K_TRY(b2k_resolve(ctx, dotv, &rd));
+    if (vout >= 0) B2K_TRY(b2k_resolve(ctx, vout, &rv));
+    if (dsub >= 0) B2K_TRY(b2k_resolve(ctx, dsub, &rs));
+    double h[4] = {*dot, xscale ? *xscale : 0.0, dsub_scale, 0.0};     // slot, xscale, dot_sub_scale, stop
+    const int32_t hstop = stop;
+    memcpy(&h[3], &hstop, sizeof(hstop));
+    double* d = nullptr;
+    B2K_CUDA(ctx, B2K_DMALLOC(&d, sizeof(h)));
+    cudaError_t e = cudaMemcpyAsync(d, h, sizeof(h), cudaMemcpyHostToDevice, ctx->stream);
+    int32_t rc = B2K_OK;
+    if (e == cudaSuccess) {
+        SpmvFuse fz;
+        memset(&fz, 0, sizeof(fz));
+        fz.xscale = xscale ? d + 1 : nullptr;
+        fz.vout = vout >= 0 ? rv.ptr : nullptr;
+        fz.stop = reinterpret_cast<const int*>(d + 3);
+        fz.dot_self = dot_self;
+        fz.l2_hints = l2_hints;
+        fz.dot_sub_vec = dsub >= 0 ? rs.ptr : nullptr;
+        fz.dot_sub_scale = dsub >= 0 ? d + 2 : nullptr;
+        rc = b2k_enqueue_apply_fused(ctx, op, rx, ry, a0, a1, shifted != 0, dotv >= 0 ? &rd : nullptr,
+                                     no_slot ? nullptr : d, &fz);
+        e = cudaMemcpyAsync(dot, d, sizeof(double), cudaMemcpyDeviceToHost, ctx->stream);
+    }
+    if (e == cudaSuccess) e = cudaStreamSynchronize(ctx->stream);
+    B2K_DFREE(d);
+    B2K_TRY(rc);
+    B2K_CUDA(ctx, e);
+    return B2K_OK;
 }
 
 // opt in to > 48 KB dynamic shared memory for the pipelined SpMV (called per context)
@@ -2246,6 +2312,7 @@ int32_t b2k_enqueue_apply_fused(b2k_ctx* ctx, const b2k_op* op, const VecRef& x,
         sa.n_rows = op->n_rows; sa.n_loc = x.n; sa.halo_lo = op->halo_lo;
         for (int i = 0; i < 7; ++i) sa.c[i] = op->sc[i];
         const int grid = (int)std::max<int64_t>(1, std::min<int64_t>((op->n_rows + 255) / 256, (int64_t)ctx->num_sms * 8));
+        g_spmv_launch[0] = 4; g_spmv_launch[1] = 0; g_spmv_launch[2] = grid; g_spmv_launch[3] = 0;
         const int pr2 = b2k_prof_begin(ctx, 0, 2.0 * ctx->esize * op->n_rows);
         if (ctx->dtype == B2K_F64)
             k_stencil_apply<double><<<grid, 256, 0, ctx->stream>>>(sa, (const double*)xsrc, (const double*)halo, (double*)y.ptr,
@@ -2271,6 +2338,8 @@ int32_t b2k_enqueue_apply_fused(b2k_ctx* ctx, const b2k_op* op, const VecRef& x,
         // the grid of k_spmv_pipe's variant: the CTA partials of the dot, and so its rounding, stay the same
         const int per_sm = g_spmv_variant == 1 ? 4 : 3;
         const int grid = std::min(op->nblk, per_sm * ctx->num_sms);
+        g_spmv_launch[0] = 3; g_spmv_launch[2] = grid; g_spmv_launch[3] = op->nblk;
+        g_spmv_launch[1] = (ctx->dtype == B2K_F32 || op->cvals ? 1 : 0) | (op->ccol ? 2 : 0);
 #define LAUNCH_C(T, VS, IS, cv, cc)                                                                            \
     k_spmv_compact<T, VS, IS><<<grid, SPP_THREADS, SpcLayout<T, VS, IS>::SMEM, ctx->stream>>>(                 \
         op->rowptr, op->colidx, (const T*)op->vals, (const VS*)(cv), (const IS*)(cc), op->crp, (const T*)xsrc, \
@@ -2287,6 +2356,7 @@ int32_t b2k_enqueue_apply_fused(b2k_ctx* ctx, const b2k_op* op, const VecRef& x,
     } else if (g_spmv_pipe) {
         const int per_sm = g_spmv_variant == 1 ? 4 : 3;
         const int grid = std::min(op->nblk, per_sm * ctx->num_sms);
+        g_spmv_launch[0] = 2; g_spmv_launch[1] = g_spmv_variant; g_spmv_launch[2] = grid; g_spmv_launch[3] = op->nblk;
 #define LAUNCH_V(T, NS, MB)                                                                    \
     k_spmv_pipe<T, NS, MB><<<grid, SPP_THREADS, SppLayout<T, NS>::SMEM, ctx->stream>>>(        \
         op->rowptr, op->colidx, (const T*)op->vals, (const T*)xsrc, (const T*)halo, n_loc,     \
@@ -2301,6 +2371,7 @@ int32_t b2k_enqueue_apply_fused(b2k_ctx* ctx, const b2k_op* op, const VecRef& x,
         }
 #undef LAUNCH_V
     } else {
+        g_spmv_launch[0] = 1; g_spmv_launch[1] = 0; g_spmv_launch[2] = op->nblk; g_spmv_launch[3] = op->nblk;
 #define LAUNCH(T)                                                                              \
     k_spmv_stream<T><<<op->nblk, SP_BT, 0, ctx->stream>>>(                                     \
         op->rowptr, op->colidx, (const T*)op->vals, (const T*)xsrc, (const T*)halo, n_loc,     \
