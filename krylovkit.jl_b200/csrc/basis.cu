@@ -1878,6 +1878,7 @@ int32_t chain_step_gs(b2k_ctx* ctx, const Panel& pn, int K1, const VecRef& rw, d
         fp.ph[1].coef = slot(PEER_CH_COEF, ps.seq_coef[0]);
         fp.ph[1].coef_sets = ps.pd.nranks;
         fp.ph[1].coef_stride = PEER_SLOT;
+        fp.ph[1].coef_ranks = 1;
         fp.fin.A = fp.ph[1].coef; fp.fin.G = ps.pd.nranks; fp.fin.stride = PEER_SLOT; fp.fin.peer = 1;
         // rows the neighbours need for their next SpMV leave with the final store
         if (ps.seq_halo) {

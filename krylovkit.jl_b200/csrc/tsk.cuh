@@ -101,6 +101,7 @@ struct PhaseParams {
     const T* coef_t;     // alternative: coefficients stored as a device vector of T
     int32_t coef_sets;
     int32_t coef_stride;
+    int32_t coef_ranks;  // the sets are per-rank sums (peer window): added in rank order (coef_ranksum)
     T alphac, betax;
     int32_t beta_mode;   // 0: hard zero, 1: one, 2: general
     // outputs
@@ -185,6 +186,17 @@ __device__ __forceinline__ double coef_colsum(const double* P, int G, int stride
                                               bool valid) {
     double a = valid ? partial_lane_sum(P + j, G, stride, l, L) : 0.0;
     for (int o = L >> 1; o > 0; o >>= 1) a += __shfl_xor_sync(0xffffffffu, a, o);
+    return a;
+}
+
+// The coefficient of column j from the nranks per-rank sums of a row-sharded launch (peer window): added in rank
+// order from 0.0 by lane 0 of the column, as peer_sum1 and the synchronous step's all-reduce add them, so that a chained
+// step has the bits of a synchronous one at any number of ranks (coef_colsum's lane tree would add ranks 0 and 2 first
+// at three ranks).  Only lane 0's value is used.
+__device__ __forceinline__ double coef_ranksum(const double* P, int G, int stride, int j, int l, bool valid) {
+    double a = 0.0;
+    if (valid && l == 0)
+        for (int g = 0; g < G; ++g) a += __ldcg(P + (size_t)g * stride + j);
     return a;
 }
 
@@ -292,7 +304,8 @@ __device__ __forceinline__ void consumer_phase(const PhaseParams<T>& p, const Sm
             const int L = coef_lanes(p.k);
             const int j = tid / L, l = tid % L;
             const bool valid = j < p.k;
-            const double h = coef_colsum(p.coef, p.coef_sets, p.coef_stride, j, l, L, valid);
+            const double h = p.coef_ranks ? coef_ranksum(p.coef, p.coef_sets, p.coef_stride, j, l, valid)
+                                          : coef_colsum(p.coef, p.coef_sets, p.coef_stride, j, l, L, valid);
             if (valid && l == 0) cs[PRO ? (j + 2) % p.k : j] = p.alphac * (T)h;
         }
         named_bar_sync(1, NCONS);
@@ -469,8 +482,9 @@ struct FinalizeParams {
     int* stop;
     unsigned* ticket;
     int enabled;
-    // row-sharded (peer window): A/B are then the per-rank sums in MY window (G = nranks, stride = PEER_SLOT),
-    // N the LOCAL per-CTA norm partials (G_local of them); the norm and <v, A v> are summed over ranks here
+    // row-sharded (peer window): A/B are then the per-rank sums in MY window (G = nranks, stride = PEER_SLOT), added in
+    // rank order (coef_ranksum), N the LOCAL per-CTA norm partials (G_local of them); the norm and <v, A v> are summed
+    // over ranks here
     int peer;
     int G_local;
 };
@@ -483,7 +497,7 @@ __device__ __forceinline__ void finalize_block(const FinalizeParams& f, int tid,
         const int L = coef_lanes(f.k);
         const int j = tid / L, l = tid % L;
         const bool valid = j < f.k;
-        double a = coef_colsum(f.A, f.G, f.stride, j, l, L, valid);
+        double a = f.peer ? coef_ranksum(f.A, f.G, f.stride, j, l, valid) : coef_colsum(f.A, f.G, f.stride, j, l, L, valid);
         if (f.B) a += coef_colsum(f.B, f.G, f.stride, j, l, L, valid);
         if (valid && l == 0) {
             if (f.res) f.res[f.off + j] = a;

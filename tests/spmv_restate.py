@@ -177,17 +177,21 @@ def dot(fma, dt, dv, sd, gid, rank, grid, kernel, plain=None):
 
 
 def apply(fma, dt, kernel, grid, x, *, csr=None, stencil=None, rowblk=None, a0=0.0, a1=1.0, shifted=False,
-          xscale=None, dotv=None, dot_self=False, dsub=None, dsc=0.0):
+          xscale=None, dotv=None, dot_self=False, dsub=None, dsc=0.0, gather=None):
     """(y, vout, dot) of one launch; csr = (rowptr, colidx, vals), stencil = (nx, ny, nz, coeffs); vout is the
-    normalised operand (what a launch with vout stores), dot is None without a dot"""
+    normalised operand (what a launch with vout stores), dot is None without a dot.
+    gather = (xg, r0): a row shard.  The rows gather from the global operand xg (CSR columns are global, the stencil is
+    the global grid's rows r0, r0 + 1, ...), and x, dotv and dsub are the shard's row-aligned slices the epilogue uses."""
     assert kernel in KERNELS
+    xg, r0 = (x, 0) if gather is None else gather
     if kernel == "stencil":
-        s = stencil_rows(*stencil, x, dt, xscale)
+        nrows = len(x) if gather is not None else int(np.prod(stencil[:3]))
+        s = stencil_rows(*stencil, xg, dt, xscale)[r0:r0 + nrows]
         gid, rank = stencil_threads(len(s), grid)
         plain = None
     else:
         rowptr, colidx, vals = csr
-        s = csr_rows(rowptr, colidx, vals, x, dt, xscale, kernel)
+        s = csr_rows(rowptr, colidx, vals, xg, dt, xscale, kernel)
         assert kernel != "stream" or grid == len(rowblk) - 1
         gid, rank = csr_threads(rowblk, grid)
         plain = (np.diff(np.asarray(rowptr, dtype=np.int64)) > SP_NNZ) if kernel == "stream" else None
