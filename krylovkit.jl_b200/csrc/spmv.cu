@@ -188,20 +188,198 @@ k_spmv_stream(const int32_t* __restrict__ rowptr, const int32_t* __restrict__ co
 // consumer warps gather x, multiply in place, and sum rows out of shared memory while the
 // next blocks are already in flight.  Same arithmetic (products rounded, summed in CSR
 // order) as k_spmv_stream, which remains as the reference implementation for tests.
-constexpr int SPP_NSTG = 3;
 constexpr int SPP_RMAX = 1024;            // rowptr entries staged per block
 constexpr int SPP_TV = SP_NNZ + 8;        // staged nonzeros (block + alignment slack)
 constexpr int SPP_CONS = 256;
 constexpr int SPP_THREADS = SPP_CONS + 32;
-template <typename T, int NSTG = SPP_NSTG> struct SppLayout {
-    static constexpr int VAL_BYTES = SPP_TV * (int)sizeof(T);
-    static constexpr int COL_BYTES = SPP_TV * 4;
-    static constexpr int RP_BYTES = (SPP_RMAX + 8) * 4;
-    static constexpr int STAGE = VAL_BYTES + COL_BYTES + RP_BYTES;
-    static constexpr int OFF_BAR = NSTG * STAGE;
+
+// A tile's bulk copies into ring stage st, completing on the stage's full barrier.
+struct TileCopy {
+    uint32_t st, bar;
+    int lane;
+    bool hints;                  // L2 evict_first: the CSR arrays are read once per apply
+    // lane 0 announces the tile's bytes before any of its copies is issued
+    __device__ __forceinline__ void expect(uint32_t bytes) const {
+        if (lane == 0) mbar_expect_tx(bar, bytes);
+        __syncwarp();
+    }
+    // lane l copies `bytes` bytes from src to stage offset off
+    __device__ __forceinline__ void operator()(int l, int off, const void* src, uint32_t bytes) const {
+        if (lane != l || bytes == 0) return;
+        if (hints) bulk_g2s_hint(st + off, src, bytes, bar, l2_policy_evict_first());
+        else bulk_g2s(st + off, src, bytes, bar);
+    }
+};
+
+// The TMA tile ring of the warp-specialised CSR kernels (k_spmv_pipe, k_spmv_compact, k_spmv_pencil, k_spmm_pipe).
+// Shared memory: NSTG stages of STAGE bytes, EXTRA bytes of the kernel's own, the stages' full and empty mbarriers,
+// then the consumers' reduction scratch red (32 doubles) and flag.  CTA b takes tiles b, b + G, ...  Per tile the
+// producer warp waits for the stage to be empty and issues the tile's copies; a tile of more than SP_NNZ nonzeros (one
+// long row) copies nothing, lane 0 arrives instead and the consumers read global memory.  The consumers wait for the
+// stage to be full, read it, and release it with one arrival per warp.
+template <int NSTG_, int STAGE_, int EXTRA = 0>
+struct TileRing {
+    static constexpr int NSTG = NSTG_, STAGE = STAGE_;
+    static constexpr int OFF_EXTRA = NSTG * STAGE;
+    static constexpr int OFF_BAR = OFF_EXTRA + EXTRA;
     static constexpr int OFF_RED = OFF_BAR + 2 * NSTG * 8 + 16;
     static constexpr int SMEM = OFF_RED + 32 * 8 + 16;
+
+    uint8_t* smem;
+    const int32_t* rowblk;
+    const int32_t* pblk;
+    int nblk;
+    uint32_t s = 0, ph = 0;              // consumers: the current tile's stage and its phase parity
+    int4 dn = make_int4(0, 0, 0, 0);     // consumers: (r0, r1, p0, p1) of the next tile
+
+    __device__ __forceinline__ uint8_t* stage(uint32_t i) const { return smem + i * STAGE; }
+    __device__ __forceinline__ uint32_t full(uint32_t i) const { return smem_u32(smem + OFF_BAR) + 8 * i; }
+    __device__ __forceinline__ uint32_t empty(uint32_t i) const { return full(NSTG + i); }
+    __device__ __forceinline__ double* red() const { return reinterpret_cast<double*>(smem + OFF_RED); }
+    __device__ __forceinline__ int* flag() const { return reinterpret_cast<int*>(smem + OFF_RED + 32 * 8); }
+    __device__ __forceinline__ int4 desc(int t) const {
+        return make_int4(rowblk[t], rowblk[t + 1], pblk[t], pblk[t + 1]);
+    }
+
+    // every thread of the CTA
+    __device__ __forceinline__ void init() const {
+        if (threadIdx.x == 0) {
+            for (int i = 0; i < NSTG; ++i) {
+                mbar_init(full(i), 1);
+                mbar_init(empty(i), SPP_CONS / 32);
+            }
+            fence_mbar_init();
+        }
+        __syncthreads();
+    }
+
+    // The producer warp: issue(copy, r0, r1, p0, p1) stages a tile of <= SP_NNZ nonzeros through copy.expect and copy.
+    template <typename Issue>
+    __device__ __forceinline__ void produce(bool hints, Issue issue) const {
+        const int lane = threadIdx.x & 31;
+        uint32_t ps = 0, pph = 0;
+        int tile = blockIdx.x;
+        int d = 0;   // lanes 0..3 hold r0, r1, p0, p1 of the current tile
+        if (tile < nblk && lane < 4) d = (lane < 2) ? rowblk[tile + lane] : pblk[tile + lane - 2];
+        for (; tile < nblk; tile += gridDim.x) {
+            const int r0 = __shfl_sync(0xffffffffu, d, 0), r1 = __shfl_sync(0xffffffffu, d, 1);
+            const int p0 = __shfl_sync(0xffffffffu, d, 2), p1 = __shfl_sync(0xffffffffu, d, 3);
+            const int nt = tile + gridDim.x;      // prefetch the next descriptor before blocking
+            if (nt < nblk && lane < 4) d = (lane < 2) ? rowblk[nt + lane] : pblk[nt + lane - 2];
+            mbar_wait(empty(ps), pph ^ 1);
+            if (p1 - p0 <= SP_NNZ) issue(TileCopy{smem_u32(stage(ps)), full(ps), lane, hints}, r0, r1, p0, p1);
+            else if (lane == 0) mbar_arrive(full(ps));
+            if (++ps == NSTG) { ps = 0; pph ^= 1; }
+        }
+    }
+
+    // The consumers: start() before the tile loop, then per tile next(tile) gives its descriptor (and loads the next
+    // one's into dn), wait() waits for its stage, release() hands the stage back and moves to the next.
+    __device__ __forceinline__ void start() {
+        if ((int)blockIdx.x < nblk) dn = desc(blockIdx.x);
+    }
+    __device__ __forceinline__ int4 next(int tile) {
+        const int4 d = dn;
+        const int nt = tile + gridDim.x;
+        if (nt < nblk) dn = desc(nt);
+        return d;
+    }
+    __device__ __forceinline__ void wait() const { mbar_wait(full(s), ph); }
+    // the next tile's stage, and a wait for it while the current one is still held
+    __device__ __forceinline__ uint32_t s_next() const { return s + 1 == NSTG ? 0 : s + 1; }
+    __device__ __forceinline__ void wait_next() const { mbar_wait(full(s_next()), s + 1 == NSTG ? ph ^ 1 : ph); }
+    // wrote: the consumers wrote the stage; their generic-proxy writes must precede its reuse by the TMA unit
+    __device__ __forceinline__ void release(bool wrote = true) {
+        if (wrote) fence_proxy_async();
+        __syncwarp();
+        if ((threadIdx.x & 31) == 0) mbar_arrive(empty(s));
+        if (++s == NSTG) { s = 0; ph ^= 1; }
+    }
 };
+
+// A ring stage of k_spmv_pipe and k_spmm_pipe (NV = 1) and k_spmv_pencil (NV = 2: A's values, then B's): NV value
+// arrays, the columns and the row pointers of a tile, each with room for the 16-byte alignment of its copy.
+template <typename T, int NV> struct CsrStage {
+    static constexpr int VAL_BYTES = SPP_TV * (int)sizeof(T);
+    static constexpr int OFF_COL = NV * VAL_BYTES;
+    static constexpr int OFF_RP = OFF_COL + SPP_TV * 4;
+    static constexpr int BYTES = OFF_RP + (SPP_RMAX + 8) * 4;
+};
+template <typename T, int NSTG, int EXTRA = 0> using SppRing = TileRing<NSTG, CsrStage<T, 1>::BYTES, EXTRA>;
+
+// A CsrStage's copies of tile (r0, r1, p0, p1): lane v copies value array v, lane NV the columns and lane NV + 1 the
+// row pointers (none for a tile of more than SPP_RMAX rows, whose consumers read rowptr from global memory).
+template <typename T, int NV>
+__device__ __forceinline__ void copy_csr_tile(const TileCopy& c, const T* const (&vals)[NV], const int32_t* colidx,
+                                              const int32_t* rowptr, int r0, int r1, int p0, int p1) {
+    using SG = CsrStage<T, NV>;
+    const int p0a = p0 & ~3, cnt = ((p1 + 3) & ~3) - p0a;
+    const int r0a = r0 & ~3;
+    const int rcnt = (r1 - r0 <= SPP_RMAX) ? (((r1 + 1 + 3) & ~3) - r0a) : 0;
+    const uint32_t vb = (uint32_t)cnt * (uint32_t)sizeof(T), cb = (uint32_t)cnt * 4u, rb = (uint32_t)rcnt * 4u;
+    c.expect(NV * vb + cb + rb);
+#pragma unroll
+    for (int v = 0; v < NV; ++v) c(v, v * SG::VAL_BYTES, vals[v] + p0a, vb);
+    c(NV, SG::OFF_COL, colidx + p0a, cb);
+    c(NV + 1, SG::OFF_RP, rowptr + r0a, rb);
+}
+
+// The fused dots of the TMA kernels, summed by their SPP_CONS consumer threads (named barrier 1): per sum k, each
+// warp's butterfly of its threads' v[k] and the warps added in order from 0.0 give the CTA partial part[k G + b]; the
+// last CTA to take a ticket has thread t add partials t, t + SPP_CONS, ... from 0.0, reduces those the same way, and
+// its thread 0 calls fin(k, total_k) for k = 0 .. NRED-1.  red and flag: the ring's scratch.
+template <int NRED, typename Fin>
+__device__ __forceinline__ void consumer_sums(const double (&v)[NRED], double* __restrict__ part,
+                                              unsigned* __restrict__ ticket, double* red, int* flag, Fin fin) {
+    constexpr int NW = SPP_CONS / 32;
+    static_assert(NRED * NW <= 32, "red holds 32 doubles");
+    const int tid = threadIdx.x, lane = tid & 31, w = tid >> 5;
+    // thread 0 gets each x[k] summed over the consumers
+    auto cta_sums = [&](double (&x)[NRED]) {
+#pragma unroll
+        for (int k = 0; k < NRED; ++k) x[k] = warp_sum(x[k]);
+        named_bar_sync(1, SPP_CONS);                    // red's last reader is done with it
+        if (lane == 0) {
+#pragma unroll
+            for (int k = 0; k < NRED; ++k) red[k * NW + w] = x[k];
+        }
+        named_bar_sync(1, SPP_CONS);
+        if (tid == 0) {
+#pragma unroll
+            for (int k = 0; k < NRED; ++k) {
+                double tot = 0.0;
+                for (int i = 0; i < NW; ++i) tot += red[k * NW + i];
+                x[k] = tot;
+            }
+        }
+    };
+    double s[NRED];
+#pragma unroll
+    for (int k = 0; k < NRED; ++k) s[k] = v[k];
+    cta_sums(s);
+    if (tid == 0) {
+#pragma unroll
+        for (int k = 0; k < NRED; ++k) part[(size_t)k * gridDim.x + blockIdx.x] = s[k];
+        __threadfence();
+        const unsigned t = atomicInc(ticket, gridDim.x - 1);
+        *flag = (t == gridDim.x - 1);
+    }
+    named_bar_sync(1, SPP_CONS);
+    if (!*flag) return;
+    __threadfence();
+    const volatile double* pv = part;
+#pragma unroll
+    for (int k = 0; k < NRED; ++k) s[k] = 0.0;
+    for (int g = tid; g < (int)gridDim.x; g += SPP_CONS) {
+#pragma unroll
+        for (int k = 0; k < NRED; ++k) s[k] += pv[(size_t)k * gridDim.x + g];
+    }
+    cta_sums(s);
+    if (tid == 0) {
+#pragma unroll
+        for (int k = 0; k < NRED; ++k) fin(k, s[k]);
+    }
+}
 
 __global__ void k_pblk(const int32_t* __restrict__ rowptr, const int32_t* __restrict__ rowblk, int count,
                        int32_t* __restrict__ pblk) {
@@ -293,62 +471,19 @@ k_spmv_pipe(const int32_t* __restrict__ rowptr, const int32_t* __restrict__ coli
             const T* __restrict__ xs, const T* __restrict__ dotv, double* __restrict__ part,
             unsigned* __restrict__ ticket, double* __restrict__ out, const SpmvFuse fz,
             const __grid_constant__ PeerStep ps) {
-    using LY = SppLayout<T, NSTG>;
+    using SG = CsrStage<T, 1>;
     extern __shared__ __align__(128) uint8_t smem[];
     if (fz.stop && *reinterpret_cast<const volatile int*>(fz.stop)) return;
-    const uint32_t full = smem_u32(smem + LY::OFF_BAR), empty = full + NSTG * 8;
-    double* red = reinterpret_cast<double*>(smem + LY::OFF_RED);
-    int* flag = reinterpret_cast<int*>(smem + LY::OFF_RED + 32 * 8);
-    if (threadIdx.x == 0) {
-        for (int i = 0; i < NSTG; ++i) {
-            mbar_init(full + 8 * i, 1);
-            mbar_init(empty + 8 * i, SPP_CONS / 32);
-        }
-        fence_mbar_init();
-    }
-    __syncthreads();
-    const int lane = threadIdx.x & 31;
-    uint32_t s = 0, ph = 0;
+    SppRing<T, NSTG> ring{smem, rowblk, pblk, nblk};
+    ring.init();
     if (threadIdx.x >= SPP_CONS) {
-        // ------------------------------ producer warp ------------------------------
-        int tile = blockIdx.x;
-        int d = 0;   // lanes 0..3 hold r0, r1, p0, p1 of the current tile
-        if (tile < nblk && lane < 4) d = (lane < 2) ? rowblk[tile + lane] : pblk[tile + lane - 2];
-        for (; tile < nblk; tile += gridDim.x) {
-            const int r0 = __shfl_sync(0xffffffffu, d, 0), r1 = __shfl_sync(0xffffffffu, d, 1);
-            const int p0 = __shfl_sync(0xffffffffu, d, 2), p1 = __shfl_sync(0xffffffffu, d, 3);
-            const int nt = tile + gridDim.x;      // prefetch the next descriptor before blocking
-            if (nt < nblk && lane < 4) d = (lane < 2) ? rowblk[nt + lane] : pblk[nt + lane - 2];
-            mbar_wait(empty + 8 * s, ph ^ 1);
-            const int nnzb = p1 - p0, nrows = r1 - r0;
-            if (nnzb <= SP_NNZ) {
-                const int p0a = p0 & ~3, cnt = ((p1 + 3) & ~3) - p0a;
-                const int r0a = r0 & ~3;
-                const int rcnt = (nrows <= SPP_RMAX) ? (((r1 + 1 + 3) & ~3) - r0a) : 0;
-                const uint32_t vb = (uint32_t)cnt * (uint32_t)sizeof(T), cb = (uint32_t)cnt * 4u,
-                               rb = (uint32_t)rcnt * 4u;
-                const uint32_t st = smem_u32(smem + s * LY::STAGE);
-                if (lane == 0) mbar_expect_tx(full + 8 * s, vb + cb + rb);
-                __syncwarp();
-                if (fz.l2_hints) {
-                    const uint64_t pol = l2_policy_evict_first();
-                    if (lane == 0 && vb) bulk_g2s_hint(st, vals + p0a, vb, full + 8 * s, pol);
-                    if (lane == 1 && cb) bulk_g2s_hint(st + LY::VAL_BYTES, colidx + p0a, cb, full + 8 * s, pol);
-                    if (lane == 2 && rb) bulk_g2s_hint(st + LY::VAL_BYTES + LY::COL_BYTES, rowptr + r0a, rb, full + 8 * s, pol);
-                } else {
-                    if (lane == 0 && vb) bulk_g2s(st, vals + p0a, vb, full + 8 * s);
-                    if (lane == 1 && cb) bulk_g2s(st + LY::VAL_BYTES, colidx + p0a, cb, full + 8 * s);
-                    if (lane == 2 && rb) bulk_g2s(st + LY::VAL_BYTES + LY::COL_BYTES, rowptr + r0a, rb, full + 8 * s);
-                }
-            } else {
-                if (lane == 0) mbar_arrive(full + 8 * s);   // long row: consumers read global memory
-            }
-            if (++s == NSTG) { s = 0; ph ^= 1; }
-        }
+        ring.produce(fz.l2_hints, [&](const TileCopy& c, int r0, int r1, int p0, int p1) {
+            copy_csr_tile<T, 1>(c, {vals}, colidx, rowptr, r0, r1, p0, p1);
+        });
         return;
     }
     // ---------------------------------- consumers ----------------------------------
-    const int tid = threadIdx.x, w = tid >> 5;
+    const int tid = threadIdx.x;
     const bool tr0 = fz.trace && blockIdx.x == 0 && tid == 0;
     if (tr0) b2k_trace(fz.trace, 1);
     if (ps.on && ps.seq_halo) {        // boundary rows of x arrive from the neighbours through the peer window;
@@ -360,19 +495,17 @@ k_spmv_pipe(const int32_t* __restrict__ rowptr, const int32_t* __restrict__ coli
     }
     if (tr0) b2k_trace(fz.trace, 2);
     RowEpilogue<T> ep{fz, x, y, xs, dotv, a0, a1, shifted};
-    int tile = blockIdx.x;
-    int4 dn = make_int4(0, 0, 0, 0);
-    if (tile < nblk) dn = make_int4(rowblk[tile], rowblk[tile + 1], pblk[tile], pblk[tile + 1]);
-    for (; tile < nblk; tile += gridDim.x) {
-        const int r0 = dn.x, r1 = dn.y, p0 = dn.z, p1 = dn.w;
-        const int nt = tile + gridDim.x;
-        if (nt < nblk) dn = make_int4(rowblk[nt], rowblk[nt + 1], pblk[nt], pblk[nt + 1]);
+    ring.start();
+    for (int tile = blockIdx.x; tile < nblk; tile += gridDim.x) {
+        const int4 d = ring.next(tile);
+        const int r0 = d.x, r1 = d.y, p0 = d.z, p1 = d.w;
         const int nnzb = p1 - p0, nrows = r1 - r0;
-        mbar_wait(full + 8 * s, ph);
+        ring.wait();
         if (nnzb <= SP_NNZ) {
-            T* vs = reinterpret_cast<T*>(smem + s * LY::STAGE);
-            const int32_t* cs = reinterpret_cast<const int32_t*>(smem + s * LY::STAGE + LY::VAL_BYTES);
-            const int32_t* rs = reinterpret_cast<const int32_t*>(smem + s * LY::STAGE + LY::VAL_BYTES + LY::COL_BYTES);
+            uint8_t* const st = ring.stage(ring.s);
+            T* vs = reinterpret_cast<T*>(st);
+            const int32_t* cs = reinterpret_cast<const int32_t*>(st + SG::OFF_COL);
+            const int32_t* rs = reinterpret_cast<const int32_t*>(st + SG::OFF_RP);
             const int p0a = p0 & ~3, r0a = r0 & ~3, off = p0 - p0a;
             constexpr int U = SP_NNZ / SPP_CONS;
             T xv[U];
@@ -406,45 +539,18 @@ k_spmv_pipe(const int32_t* __restrict__ rowptr, const int32_t* __restrict__ coli
                 ep.row(r, ld, sum);
             }
         } else {
-            ep.long_row(r0, vals, colidx, p0, nnzb, red,
+            ep.long_row(r0, vals, colidx, p0, nnzb, ring.red(),
                         [&](int32_t cc) { return (cc < n_loc) ? __ldg(x + cc) : __ldg(halo + (cc - n_loc)); });
         }
-        fence_proxy_async();   // generic-proxy writes to the stage precede its reuse by the TMA unit
-        __syncwarp();
-        if (lane == 0) mbar_arrive(empty + 8 * s);
-        if (++s == NSTG) { s = 0; ph ^= 1; }
+        ring.release();
     }
     if (tr0) b2k_trace(fz.trace, 3);
     if (ep.want_dot) {
-        double v = warp_sum((double)ep.dacc);
-        if (lane == 0) red[w] = v;
-        named_bar_sync(1, SPP_CONS);
-        if (tid == 0) {
-            double tot = 0.0;
-            for (int i = 0; i < SPP_CONS / 32; ++i) tot += red[i];
-            part[blockIdx.x] = tot;
-            __threadfence();
-            const unsigned t = atomicInc(ticket, gridDim.x - 1);
-            *flag = (t == gridDim.x - 1);
-        }
-        named_bar_sync(1, SPP_CONS);
-        if (*flag) {
-            __threadfence();
-            double v2 = 0.0;
-            const volatile double* pv = part;
-            for (int g = tid; g < (int)gridDim.x; g += SPP_CONS) v2 += pv[g];
-            v2 = warp_sum(v2);
-            named_bar_sync(1, SPP_CONS);
-            if (lane == 0) red[w] = v2;
-            named_bar_sync(1, SPP_CONS);
-            if (tid == 0) {
-                double tot = 0.0;
-                for (int i = 0; i < SPP_CONS / 32; ++i) tot += red[i];
-                *out = tot;
-                if (ps.on && ps.seq_alpha) peer_publish1(ps.pd, PEER_CH_ALPHA, ps.seq_alpha, tot);
-                if (fz.trace) b2k_trace(fz.trace, 4);
-            }
-        }
+        consumer_sums<1>({(double)ep.dacc}, part, ticket, ring.red(), ring.flag(), [&](int, double tot) {
+            *out = tot;
+            if (ps.on && ps.seq_alpha) peer_publish1(ps.pd, PEER_CH_ALPHA, ps.seq_alpha, tot);
+            if (fz.trace) b2k_trace(fz.trace, 4);
+        });
     }
 }
 
@@ -472,14 +578,10 @@ template <typename T, typename VS, typename IS> struct SpcLayout {
     static constexpr int COL_BYTES = SPC_TV * (int)sizeof(IS);
     static constexpr int RP_BYTES = (SPP_RMAX + 16) * 2;
     static constexpr int STAGE = VAL_BYTES + COL_BYTES + RP_BYTES;
-    static constexpr int PROD_BYTES = PROD ? SP_NNZ * (int)sizeof(T) : 0;
-    static constexpr int TAIL = 2 * 4 * 8 + 16 + 32 * 8 + 16;            // barriers of up to 4 stages, red, flag
-    static constexpr int NSTG = std::min(4, (SPC_SMEM_MAX - PROD_BYTES - TAIL) / STAGE);
-    static constexpr int OFF_PROD = NSTG * STAGE;
-    static constexpr int OFF_BAR = OFF_PROD + PROD_BYTES;
-    static constexpr int OFF_RED = OFF_BAR + 2 * NSTG * 8 + 16;
-    static constexpr int SMEM = OFF_RED + 32 * 8 + 16;
-    static_assert(NSTG >= 2 && SMEM <= SPC_SMEM_MAX, "compact SpMV stage ring does not fit 4 CTAs per SM");
+    static constexpr int PROD_BYTES = PROD ? SP_NNZ * (int)sizeof(T) : 0;       // the ring's EXTRA bytes
+    static constexpr int NSTG = std::min(4, (SPC_SMEM_MAX - PROD_BYTES - TileRing<4, 0>::SMEM) / STAGE);
+    using Ring = TileRing<NSTG, STAGE, PROD_BYTES>;
+    static_assert(NSTG >= 2 && Ring::SMEM <= SPC_SMEM_MAX, "compact SpMV stage ring does not fit 4 CTAs per SM");
     static_assert(VAL_BYTES % 16 == 0 && COL_BYTES % 16 == 0 && RP_BYTES % 16 == 0, "TMA needs 16-byte offsets");
 };
 
@@ -492,62 +594,26 @@ k_spmv_compact(const int32_t* __restrict__ rowptr, const int32_t* __restrict__ c
                const T* __restrict__ dotv, double* __restrict__ part, unsigned* __restrict__ ticket,
                double* __restrict__ out, const SpmvFuse fz) {
     using LY = SpcLayout<T, VS, IS>;
-    constexpr int NSTG = LY::NSTG;
     constexpr bool OFFS = sizeof(IS) == 2;     // columns staged as offsets from the tile's first row
     extern __shared__ __align__(128) uint8_t smem[];
     if (fz.stop && *reinterpret_cast<const volatile int*>(fz.stop)) return;
-    const uint32_t full = smem_u32(smem + LY::OFF_BAR), empty = full + NSTG * 8;
-    double* red = reinterpret_cast<double*>(smem + LY::OFF_RED);
-    int* flag = reinterpret_cast<int*>(smem + LY::OFF_RED + 32 * 8);
-    if (threadIdx.x == 0) {
-        for (int i = 0; i < NSTG; ++i) {
-            mbar_init(full + 8 * i, 1);
-            mbar_init(empty + 8 * i, SPP_CONS / 32);
-        }
-        fence_mbar_init();
-    }
-    __syncthreads();
-    const int lane = threadIdx.x & 31;
-    uint32_t s = 0, ph = 0;
+    typename LY::Ring ring{smem, rowblk, pblk, nblk};
+    ring.init();
     if (threadIdx.x >= SPP_CONS) {
-        // ------------------------------ producer warp ------------------------------
-        int tile = blockIdx.x;
-        int d = 0;
-        if (tile < nblk && lane < 4) d = (lane < 2) ? rowblk[tile + lane] : pblk[tile + lane - 2];
-        for (; tile < nblk; tile += gridDim.x) {
-            const int r0 = __shfl_sync(0xffffffffu, d, 0), r1 = __shfl_sync(0xffffffffu, d, 1);
-            const int p0 = __shfl_sync(0xffffffffu, d, 2), p1 = __shfl_sync(0xffffffffu, d, 3);
-            const int nt = tile + gridDim.x;
-            if (nt < nblk && lane < 4) d = (lane < 2) ? rowblk[nt + lane] : pblk[nt + lane - 2];
-            mbar_wait(empty + 8 * s, ph ^ 1);
-            const int nnzb = p1 - p0, nrows = r1 - r0;
-            if (nnzb <= SP_NNZ) {
-                const int pv = al_dn<VS>(p0), pc = al_dn<IS>(p0), r0a = al_dn<uint16_t>(r0);
-                const uint32_t vb = (uint32_t)(al_up<VS>(p1) - pv) * (uint32_t)sizeof(VS);
-                const uint32_t cb = (uint32_t)(al_up<IS>(p1) - pc) * (uint32_t)sizeof(IS);
-                const uint32_t rb = nrows <= SPP_RMAX ? (uint32_t)(al_up<uint16_t>(r1 + 1) - r0a) * 2u : 0u;
-                const uint32_t st = smem_u32(smem + s * LY::STAGE);
-                if (lane == 0) mbar_expect_tx(full + 8 * s, vb + cb + rb);
-                __syncwarp();
-                if (fz.l2_hints) {
-                    const uint64_t pol = l2_policy_evict_first();
-                    if (lane == 0 && vb) bulk_g2s_hint(st, cvals + pv, vb, full + 8 * s, pol);
-                    if (lane == 1 && cb) bulk_g2s_hint(st + LY::VAL_BYTES, ccol + pc, cb, full + 8 * s, pol);
-                    if (lane == 2 && rb) bulk_g2s_hint(st + LY::VAL_BYTES + LY::COL_BYTES, crp + r0a, rb, full + 8 * s, pol);
-                } else {
-                    if (lane == 0 && vb) bulk_g2s(st, cvals + pv, vb, full + 8 * s);
-                    if (lane == 1 && cb) bulk_g2s(st + LY::VAL_BYTES, ccol + pc, cb, full + 8 * s);
-                    if (lane == 2 && rb) bulk_g2s(st + LY::VAL_BYTES + LY::COL_BYTES, crp + r0a, rb, full + 8 * s);
-                }
-            } else {
-                if (lane == 0) mbar_arrive(full + 8 * s);   // long row: consumers read global memory
-            }
-            if (++s == NSTG) { s = 0; ph ^= 1; }
-        }
+        ring.produce(fz.l2_hints, [&](const TileCopy& c, int r0, int r1, int p0, int p1) {
+            const int pv = al_dn<VS>(p0), pc = al_dn<IS>(p0), r0a = al_dn<uint16_t>(r0);
+            const uint32_t vb = (uint32_t)(al_up<VS>(p1) - pv) * (uint32_t)sizeof(VS);
+            const uint32_t cb = (uint32_t)(al_up<IS>(p1) - pc) * (uint32_t)sizeof(IS);
+            const uint32_t rb = r1 - r0 <= SPP_RMAX ? (uint32_t)(al_up<uint16_t>(r1 + 1) - r0a) * 2u : 0u;
+            c.expect(vb + cb + rb);
+            c(0, 0, cvals + pv, vb);
+            c(1, LY::VAL_BYTES, ccol + pc, cb);
+            c(2, LY::VAL_BYTES + LY::COL_BYTES, crp + r0a, rb);
+        });
         return;
     }
     // ---------------------------------- consumers ----------------------------------
-    const int tid = threadIdx.x, w = tid >> 5;
+    const int tid = threadIdx.x;
     const bool tr0 = fz.trace && blockIdx.x == 0 && tid == 0;
     if (tr0) b2k_trace(fz.trace, 1);
     if (tr0) b2k_trace(fz.trace, 2);
@@ -558,7 +624,7 @@ k_spmv_compact(const int32_t* __restrict__ rowptr, const int32_t* __restrict__ c
     T xv[U];
     auto gather = [&](uint32_t sg, int4 d) {
         if (d.w - d.z > SP_NNZ) return;
-        const IS* cg = reinterpret_cast<const IS*>(smem + sg * LY::STAGE + LY::VAL_BYTES);
+        const IS* cg = reinterpret_cast<const IS*>(ring.stage(sg) + LY::VAL_BYTES);
         const int og = d.z - al_dn<IS>(d.z);
 #pragma unroll
         for (int u = 0; u < U; ++u) {
@@ -566,27 +632,23 @@ k_spmv_compact(const int32_t* __restrict__ rowptr, const int32_t* __restrict__ c
             if (i < d.w - d.z) xv[u] = __ldg(x + (OFFS ? d.x + (int)cg[og + i] : (int)cg[og + i]));
         }
     };
-    int tile = blockIdx.x;
-    int4 dn = make_int4(0, 0, 0, 0);
-    if (tile < nblk) {
-        dn = make_int4(rowblk[tile], rowblk[tile + 1], pblk[tile], pblk[tile + 1]);
-        mbar_wait(full, 0);
-        gather(0, dn);
+    ring.start();
+    if ((int)blockIdx.x < nblk) {
+        ring.wait();
+        gather(ring.s, ring.dn);
     }
-    for (; tile < nblk; tile += gridDim.x) {
-        const int r0 = dn.x, r1 = dn.y, p0 = dn.z, p1 = dn.w;
-        const int nt = tile + gridDim.x;
-        if (nt < nblk) dn = make_int4(rowblk[nt], rowblk[nt + 1], pblk[nt], pblk[nt + 1]);
+    for (int tile = blockIdx.x; tile < nblk; tile += gridDim.x) {
+        const int4 d = ring.next(tile);
+        const int r0 = d.x, r1 = d.y, p0 = d.z, p1 = d.w;
         const int nnzb = p1 - p0, nrows = r1 - r0;
-        const uint32_t s1 = s + 1 == NSTG ? 0 : s + 1, ph1 = s + 1 == NSTG ? ph ^ 1 : ph;
         auto prefetch_next = [&]() {
-            if (nt < nblk) {
-                mbar_wait(full + 8 * s1, ph1);
-                gather(s1, dn);
+            if (tile + (int)gridDim.x < nblk) {
+                ring.wait_next();
+                gather(ring.s_next(), ring.dn);
             }
         };
         if (nnzb <= SP_NNZ) {
-            uint8_t* const st = smem + s * LY::STAGE;
+            uint8_t* const st = ring.stage(ring.s);
             VS* vs = reinterpret_cast<VS*>(st);
             const uint16_t* rs = reinterpret_cast<const uint16_t*>(st + LY::VAL_BYTES + LY::COL_BYTES);
             const int offv = p0 - al_dn<VS>(p0), r0a = al_dn<uint16_t>(r0);
@@ -596,7 +658,7 @@ k_spmv_compact(const int32_t* __restrict__ rowptr, const int32_t* __restrict__ c
             }
             T* pr;
             if constexpr (LY::PROD) {
-                pr = reinterpret_cast<T*>(smem + LY::OFF_PROD);
+                pr = reinterpret_cast<T*>(smem + LY::Ring::OFF_EXTRA);
                 named_bar_sync(1, SPP_CONS);                   // every row sum of the previous tile has read it
             } else {
                 pr = reinterpret_cast<T*>(vs) + offv;          // in place, as k_spmv_pipe
@@ -624,45 +686,17 @@ k_spmv_compact(const int32_t* __restrict__ rowptr, const int32_t* __restrict__ c
                 ep.row(r, ld, sum);
             }
         } else {
-            ep.long_row(r0, vals, colidx, p0, nnzb, red, [&](int32_t c) { return __ldg(x + c); });
+            ep.long_row(r0, vals, colidx, p0, nnzb, ring.red(), [&](int32_t c) { return __ldg(x + c); });
             prefetch_next();
         }
-        fence_proxy_async();   // generic-proxy writes to the stage precede its reuse by the TMA unit
-        __syncwarp();
-        if (lane == 0) mbar_arrive(empty + 8 * s);
-        s = s1;
-        ph = ph1;
+        ring.release();
     }
     if (tr0) b2k_trace(fz.trace, 3);
     if (ep.want_dot) {
-        double v = warp_sum((double)ep.dacc);
-        if (lane == 0) red[w] = v;
-        named_bar_sync(1, SPP_CONS);
-        if (tid == 0) {
-            double tot = 0.0;
-            for (int i = 0; i < SPP_CONS / 32; ++i) tot += red[i];
-            part[blockIdx.x] = tot;
-            __threadfence();
-            const unsigned t = atomicInc(ticket, gridDim.x - 1);
-            *flag = (t == gridDim.x - 1);
-        }
-        named_bar_sync(1, SPP_CONS);
-        if (*flag) {
-            __threadfence();
-            double v2 = 0.0;
-            const volatile double* pv = part;
-            for (int g = tid; g < (int)gridDim.x; g += SPP_CONS) v2 += pv[g];
-            v2 = warp_sum(v2);
-            named_bar_sync(1, SPP_CONS);
-            if (lane == 0) red[w] = v2;
-            named_bar_sync(1, SPP_CONS);
-            if (tid == 0) {
-                double tot = 0.0;
-                for (int i = 0; i < SPP_CONS / 32; ++i) tot += red[i];
-                *out = tot;
-                if (fz.trace) b2k_trace(fz.trace, 4);
-            }
-        }
+        consumer_sums<1>({(double)ep.dacc}, part, ticket, ring.red(), ring.flag(), [&](int, double tot) {
+            *out = tot;
+            if (fz.trace) b2k_trace(fz.trace, 4);
+        });
     }
 }
 
@@ -700,8 +734,8 @@ __global__ void k_csr_compact(const int32_t* __restrict__ rowptr, const int32_t*
 // ---------------------------------------------------------------------------------------
 // Fused two-operator SpMV of a pencil (A, B) whose CSR patterns are equal (b2k_pencil_apply / b2k_pencil_rayleigh):
 // golubyerecurrence's product `av, bv = genapply(f, v); w = add!!(av, bv, -ρ)` (golubye.jl:198-199, plus
-// `add!!(w, V[end-1], -β)` of :202/:211) and the genapply of the Ritz loop (:112-114).  k_spmv_pipe's structure with
-// B's values staged next to A's in every ring stage: rowptr and colidx are streamed once, x[c] is gathered once per
+// `add!!(w, V[end-1], -β)` of :202/:211) and the genapply of the Ritz loop (:112-114).  k_spmv_pipe's TileRing with
+// B's values staged next to A's in every stage (CsrStage<T, 2>): rowptr and colidx are streamed once, x[c] is gathered once per
 // nonzero for both products, and only the outputs are written — 2 (sizeof(T) + 2) nnz + 4 (n + 1) + 3 sizeof(T) n
 // bytes instead of 2 (sizeof(T) + 4) nnz + 8 (n + 1) + ... for the composition.
 //
@@ -712,25 +746,15 @@ __global__ void k_csr_compact(const int32_t* __restrict__ rowptr, const int32_t*
 //   MODE 1: ax = A x;  bx = B x;
 // so ax, bx and w are bit-identical to b2k_op_apply with A and with B followed by b2k_vec_axpby(w, bx, -rho, 1) and
 // b2k_vec_axpby(w, vprev, -beta, 1).  The dots (<x, w>; <x, ax> and <x, bx>) are fma chains in T over each thread's
-// rows, summed per CTA in double (warp butterflies, then the warps in order); the last CTA to take a ticket adds the
-// CTA partials in CTA order (the scheme of b2k_op_apply_dot, no FP atomics).  They may differ from b2k_vec_inner in
+// rows, summed by consumer_sums as k_spmv_pipe's dot is: per CTA in double (warp butterflies, then the warps in order),
+// then the last CTA to take a ticket adds the CTA partials in CTA order (no FP atomics).  They may differ from b2k_vec_inner in
 // the last bits.
 //
 // A stage holds both value arrays: 35008 B in Float64 (22656 B in Float32), so two stages are 70 KB (45 KB) per CTA.
 // Float64 runs 3 CTAs per SM (210 KB; four would need 280 KB of the 227 KB), Float32 4 CTAs per SM (181 KB), the
 // shape of the default single-operator variant.  -Xptxas -v: no spills for either.
-template <typename T, int NSTG> struct PenLayout {
-    static constexpr int VAL_BYTES = SPP_TV * (int)sizeof(T);
-    static constexpr int COL_BYTES = SPP_TV * 4;
-    static constexpr int RP_BYTES = (SPP_RMAX + 8) * 4;
-    static constexpr int OFF_COL = 2 * VAL_BYTES;
-    static constexpr int OFF_RP = 2 * VAL_BYTES + COL_BYTES;
-    static constexpr int STAGE = 2 * VAL_BYTES + COL_BYTES + RP_BYTES;
-    static constexpr int OFF_BAR = NSTG * STAGE;
-    static constexpr int OFF_RED = OFF_BAR + 2 * NSTG * 8 + 16;
-    static constexpr int SMEM = OFF_RED + 32 * 8 + 16;
-};
 constexpr int PEN_NSTG = 2;
+template <typename T> using PenRing = TileRing<PEN_NSTG, CsrStage<T, 2>::BYTES>;
 template <typename T> struct PenCtas { static constexpr int N = sizeof(T) == 8 ? 3 : 4; };
 
 template <typename T, int MODE>
@@ -760,81 +784,35 @@ k_spmv_pencil(const int32_t* __restrict__ rowptr, const int32_t* __restrict__ co
               const int32_t* __restrict__ rowblk, const int32_t* __restrict__ pblk, int nblk, T nrho,
               const T* __restrict__ vprev, T nbeta, int want_dot, int l2_hints, double* __restrict__ part,
               unsigned* __restrict__ ticket, double* __restrict__ out) {
-    using LY = PenLayout<T, NSTG>;
+    using SG = CsrStage<T, 2>;
     extern __shared__ __align__(128) uint8_t smem[];
-    const uint32_t full = smem_u32(smem + LY::OFF_BAR), empty = full + NSTG * 8;
-    double* red = reinterpret_cast<double*>(smem + LY::OFF_RED);
-    int* flag = reinterpret_cast<int*>(smem + LY::OFF_RED + 32 * 8);
-    if (threadIdx.x == 0) {
-        for (int i = 0; i < NSTG; ++i) {
-            mbar_init(full + 8 * i, 1);
-            mbar_init(empty + 8 * i, SPP_CONS / 32);
-        }
-        fence_mbar_init();
-    }
-    __syncthreads();
-    const int lane = threadIdx.x & 31;
-    uint32_t s = 0, ph = 0;
+    TileRing<NSTG, SG::BYTES> ring{smem, rowblk, pblk, nblk};
+    ring.init();
     if (threadIdx.x >= SPP_CONS) {
-        // ------------------------------ producer warp (k_spmv_pipe's, plus B's values) ------------------------------
-        int tile = blockIdx.x;
-        int d = 0;
-        if (tile < nblk && lane < 4) d = (lane < 2) ? rowblk[tile + lane] : pblk[tile + lane - 2];
-        for (; tile < nblk; tile += gridDim.x) {
-            const int r0 = __shfl_sync(0xffffffffu, d, 0), r1 = __shfl_sync(0xffffffffu, d, 1);
-            const int p0 = __shfl_sync(0xffffffffu, d, 2), p1 = __shfl_sync(0xffffffffu, d, 3);
-            const int nt = tile + gridDim.x;
-            if (nt < nblk && lane < 4) d = (lane < 2) ? rowblk[nt + lane] : pblk[nt + lane - 2];
-            mbar_wait(empty + 8 * s, ph ^ 1);
-            const int nnzb = p1 - p0, nrows = r1 - r0;
-            if (nnzb <= SP_NNZ) {
-                const int p0a = p0 & ~3, cnt = ((p1 + 3) & ~3) - p0a;
-                const int r0a = r0 & ~3;
-                const int rcnt = (nrows <= SPP_RMAX) ? (((r1 + 1 + 3) & ~3) - r0a) : 0;
-                const uint32_t vbyt = (uint32_t)cnt * (uint32_t)sizeof(T), cb = (uint32_t)cnt * 4u,
-                               rb = (uint32_t)rcnt * 4u;
-                const uint32_t st = smem_u32(smem + s * LY::STAGE);
-                if (lane == 0) mbar_expect_tx(full + 8 * s, 2 * vbyt + cb + rb);
-                __syncwarp();
-                if (l2_hints) {
-                    const uint64_t pol = l2_policy_evict_first();
-                    if (lane == 0 && vbyt) bulk_g2s_hint(st, va + p0a, vbyt, full + 8 * s, pol);
-                    if (lane == 3 && vbyt) bulk_g2s_hint(st + LY::VAL_BYTES, vb + p0a, vbyt, full + 8 * s, pol);
-                    if (lane == 1 && cb) bulk_g2s_hint(st + LY::OFF_COL, colidx + p0a, cb, full + 8 * s, pol);
-                    if (lane == 2 && rb) bulk_g2s_hint(st + LY::OFF_RP, rowptr + r0a, rb, full + 8 * s, pol);
-                } else {
-                    if (lane == 0 && vbyt) bulk_g2s(st, va + p0a, vbyt, full + 8 * s);
-                    if (lane == 3 && vbyt) bulk_g2s(st + LY::VAL_BYTES, vb + p0a, vbyt, full + 8 * s);
-                    if (lane == 1 && cb) bulk_g2s(st + LY::OFF_COL, colidx + p0a, cb, full + 8 * s);
-                    if (lane == 2 && rb) bulk_g2s(st + LY::OFF_RP, rowptr + r0a, rb, full + 8 * s);
-                }
-            } else {
-                if (lane == 0) mbar_arrive(full + 8 * s);   // long row: consumers read global memory
-            }
-            if (++s == NSTG) { s = 0; ph ^= 1; }
-        }
+        ring.produce(l2_hints != 0, [&](const TileCopy& c, int r0, int r1, int p0, int p1) {
+            copy_csr_tile<T, 2>(c, {va, vb}, colidx, rowptr, r0, r1, p0, p1);
+        });
         return;
     }
     // ---------------------------------- consumers ----------------------------------
-    const int tid = threadIdx.x, w = tid >> 5;
+    const int tid = threadIdx.x, lane = tid & 31, w = tid >> 5;
     const bool has_prev = MODE == 0 && vprev != nullptr;
     const bool hints = l2_hints != 0;
     const uint64_t pol_last = hints ? l2_policy_evict_last() : 0;
+    double* red = ring.red();
     T d0 = (T)0, d1 = (T)0;
-    int tile = blockIdx.x;
-    int4 dn = make_int4(0, 0, 0, 0);
-    if (tile < nblk) dn = make_int4(rowblk[tile], rowblk[tile + 1], pblk[tile], pblk[tile + 1]);
-    for (; tile < nblk; tile += gridDim.x) {
-        const int r0 = dn.x, r1 = dn.y, p0 = dn.z, p1 = dn.w;
-        const int nt = tile + gridDim.x;
-        if (nt < nblk) dn = make_int4(rowblk[nt], rowblk[nt + 1], pblk[nt], pblk[nt + 1]);
+    ring.start();
+    for (int tile = blockIdx.x; tile < nblk; tile += gridDim.x) {
+        const int4 d = ring.next(tile);
+        const int r0 = d.x, r1 = d.y, p0 = d.z, p1 = d.w;
         const int nnzb = p1 - p0, nrows = r1 - r0;
-        mbar_wait(full + 8 * s, ph);
+        ring.wait();
         if (nnzb <= SP_NNZ) {
-            T* as = reinterpret_cast<T*>(smem + s * LY::STAGE);
-            T* bs = reinterpret_cast<T*>(smem + s * LY::STAGE + LY::VAL_BYTES);
-            const int32_t* cs = reinterpret_cast<const int32_t*>(smem + s * LY::STAGE + LY::OFF_COL);
-            const int32_t* rs = reinterpret_cast<const int32_t*>(smem + s * LY::STAGE + LY::OFF_RP);
+            uint8_t* const st = ring.stage(ring.s);
+            T* as = reinterpret_cast<T*>(st);
+            T* bs = reinterpret_cast<T*>(st + SG::VAL_BYTES);
+            const int32_t* cs = reinterpret_cast<const int32_t*>(st + SG::OFF_COL);
+            const int32_t* rs = reinterpret_cast<const int32_t*>(st + SG::OFF_RP);
             const int p0a = p0 & ~3, r0a = r0 & ~3, off = p0 - p0a;
             constexpr int U = SP_NNZ / SPP_CONS;
             T xv[U];
@@ -891,53 +869,11 @@ k_spmv_pencil(const int32_t* __restrict__ rowptr, const int32_t* __restrict__ co
             }
             named_bar_sync(1, SPP_CONS);
         }
-        fence_proxy_async();   // generic-proxy writes to the stage precede its reuse by the TMA unit
-        __syncwarp();
-        if (lane == 0) mbar_arrive(empty + 8 * s);
-        if (++s == NSTG) { s = 0; ph ^= 1; }
+        ring.release();
     }
     if (want_dot) {
-        const double v0 = warp_sum((double)d0), v1 = warp_sum((double)d1);
-        if (lane == 0) {
-            red[w] = v0;
-            red[8 + w] = v1;
-        }
-        named_bar_sync(1, SPP_CONS);
-        if (tid == 0) {
-            double t0 = 0.0, t1 = 0.0;
-            for (int i = 0; i < SPP_CONS / 32; ++i) t0 += red[i];
-            for (int i = 0; i < SPP_CONS / 32; ++i) t1 += red[8 + i];
-            part[blockIdx.x] = t0;
-            part[gridDim.x + blockIdx.x] = t1;
-            __threadfence();
-            const unsigned t = atomicInc(ticket, gridDim.x - 1);
-            *flag = (t == gridDim.x - 1);
-        }
-        named_bar_sync(1, SPP_CONS);
-        if (*flag) {
-            __threadfence();
-            double a0 = 0.0, a1 = 0.0;
-            const volatile double* pv = part;
-            for (int g = tid; g < (int)gridDim.x; g += SPP_CONS) {
-                a0 += pv[g];
-                a1 += pv[gridDim.x + g];
-            }
-            a0 = warp_sum(a0);
-            a1 = warp_sum(a1);
-            named_bar_sync(1, SPP_CONS);
-            if (lane == 0) {
-                red[w] = a0;
-                red[8 + w] = a1;
-            }
-            named_bar_sync(1, SPP_CONS);
-            if (tid == 0) {
-                double t0 = 0.0, t1 = 0.0;
-                for (int i = 0; i < SPP_CONS / 32; ++i) t0 += red[i];
-                for (int i = 0; i < SPP_CONS / 32; ++i) t1 += red[8 + i];
-                out[0] = t0;
-                out[1] = t1;
-            }
-        }
+        consumer_sums<2>({(double)d0, (double)d1}, part, ticket, red, ring.flag(),
+                         [&](int k, double tot) { out[k] = tot; });
     }
 }
 
@@ -950,19 +886,14 @@ __global__ void k_pattern_diff(const int32_t* __restrict__ a, const int32_t* __r
         }
 }
 
-// SpMM for apply(A, ::Block) (blocklanczos.jl:38): the nonzero stream of a row block is staged ONCE (same TMA
-// ring as k_spmv_pipe) and used for all p <= 8 vectors of the block: 12*nnz + p*16n bytes instead of
+// SpMM for apply(A, ::Block) (blocklanczos.jl:38): the nonzero stream of a row block is staged ONCE (k_spmv_pipe's
+// stage in a 2-stage TileRing, copied without L2 hints) and used for all p <= 8 vectors of the block: 12*nnz + p*16n bytes instead of
 // p*(12*nnz + 16n).  Per vector the consumers do what k_spmv_pipe does — thread <-> nonzero gathers x_i and writes the
 // rounded product into a product buffer (two of them, alternating, so one barrier per vector), thread <-> row sums
 // its products in CSR order — bit-identical to p single-vector applies.  (The first version let one thread per row
 // walk its nonzeros for all p vectors: a fifth of the gathers in flight — slower than four SpMVs.)
 constexpr int SPM_NSTG = 2;
-template <typename T> struct SpmLayout {
-    using LY = SppLayout<T, SPM_NSTG>;
-    static constexpr int OFF_PROD = LY::SMEM;                              // two product buffers
-    static constexpr int PROD_BYTES = SPP_TV * (int)sizeof(T);
-    static constexpr int SMEM = OFF_PROD + 2 * PROD_BYTES;
-};
+template <typename T> using SpmRing = SppRing<T, SPM_NSTG, 2 * CsrStage<T, 1>::VAL_BYTES>;    // two product buffers
 constexpr int SPM_PMAX = 8;
 struct SpmmCols {
     int32_t x[SPM_PMAX], y[SPM_PMAX];
@@ -973,66 +904,31 @@ __global__ void __launch_bounds__(SPP_THREADS, 3)
 k_spmm_pipe(const int32_t* __restrict__ rowptr, const int32_t* __restrict__ colidx, const T* __restrict__ vals,
             T* __restrict__ base, int64_t ld, const __grid_constant__ SpmmCols cols, int np,
             const int32_t* __restrict__ rowblk, const int32_t* __restrict__ pblk, int nblk) {
-    using LY = SppLayout<T, SPM_NSTG>;
+    using SG = CsrStage<T, 1>;
     extern __shared__ __align__(128) uint8_t smem[];
-    const uint32_t full = smem_u32(smem + LY::OFF_BAR), empty = full + SPM_NSTG * 8;
-    double* red = reinterpret_cast<double*>(smem + LY::OFF_RED);
-    if (threadIdx.x == 0) {
-        for (int i = 0; i < SPM_NSTG; ++i) {
-            mbar_init(full + 8 * i, 1);
-            mbar_init(empty + 8 * i, SPP_CONS / 32);
-        }
-        fence_mbar_init();
-    }
-    __syncthreads();
-    const int lane = threadIdx.x & 31;
-    uint32_t s = 0, ph = 0;
+    SpmRing<T> ring{smem, rowblk, pblk, nblk};
+    ring.init();
     if (threadIdx.x >= SPP_CONS) {
-        // producer warp: identical to k_spmv_pipe
-        int tile = blockIdx.x;
-        int d = 0;
-        if (tile < nblk && lane < 4) d = (lane < 2) ? rowblk[tile + lane] : pblk[tile + lane - 2];
-        for (; tile < nblk; tile += gridDim.x) {
-            const int r0 = __shfl_sync(0xffffffffu, d, 0), r1 = __shfl_sync(0xffffffffu, d, 1);
-            const int p0 = __shfl_sync(0xffffffffu, d, 2), p1 = __shfl_sync(0xffffffffu, d, 3);
-            const int nt = tile + gridDim.x;
-            if (nt < nblk && lane < 4) d = (lane < 2) ? rowblk[nt + lane] : pblk[nt + lane - 2];
-            mbar_wait(empty + 8 * s, ph ^ 1);
-            const int nnzb = p1 - p0, nrows = r1 - r0;
-            if (nnzb <= SP_NNZ) {
-                const int p0a = p0 & ~3, cnt = ((p1 + 3) & ~3) - p0a;
-                const int r0a = r0 & ~3;
-                const int rcnt = (nrows <= SPP_RMAX) ? (((r1 + 1 + 3) & ~3) - r0a) : 0;
-                const uint32_t vb = (uint32_t)cnt * (uint32_t)sizeof(T), cb = (uint32_t)cnt * 4u, rb = (uint32_t)rcnt * 4u;
-                const uint32_t st = smem_u32(smem + s * LY::STAGE);
-                if (lane == 0) mbar_expect_tx(full + 8 * s, vb + cb + rb);
-                __syncwarp();
-                if (lane == 0 && vb) bulk_g2s(st, vals + p0a, vb, full + 8 * s);
-                if (lane == 1 && cb) bulk_g2s(st + LY::VAL_BYTES, colidx + p0a, cb, full + 8 * s);
-                if (lane == 2 && rb) bulk_g2s(st + LY::VAL_BYTES + LY::COL_BYTES, rowptr + r0a, rb, full + 8 * s);
-            } else {
-                if (lane == 0) mbar_arrive(full + 8 * s);
-            }
-            if (++s == SPM_NSTG) { s = 0; ph ^= 1; }
-        }
+        ring.produce(false, [&](const TileCopy& c, int r0, int r1, int p0, int p1) {
+            copy_csr_tile<T, 1>(c, {vals}, colidx, rowptr, r0, r1, p0, p1);
+        });
         return;
     }
-    const int tid = threadIdx.x, w = tid >> 5;
+    const int tid = threadIdx.x, lane = tid & 31, w = tid >> 5;
+    double* red = ring.red();
     auto xcol = [&](int i) -> const T* { return base + (int64_t)cols.x[i] * ld; };
     auto ycol = [&](int i) -> T* { return base + (int64_t)cols.y[i] * ld; };
-    int tile = blockIdx.x;
-    int4 dn = make_int4(0, 0, 0, 0);
-    if (tile < nblk) dn = make_int4(rowblk[tile], rowblk[tile + 1], pblk[tile], pblk[tile + 1]);
-    for (; tile < nblk; tile += gridDim.x) {
-        const int r0 = dn.x, r1 = dn.y, p0 = dn.z, p1 = dn.w;
-        const int nt = tile + gridDim.x;
-        if (nt < nblk) dn = make_int4(rowblk[nt], rowblk[nt + 1], pblk[nt], pblk[nt + 1]);
+    ring.start();
+    for (int tile = blockIdx.x; tile < nblk; tile += gridDim.x) {
+        const int4 d = ring.next(tile);
+        const int r0 = d.x, r1 = d.y, p0 = d.z, p1 = d.w;
         const int nnzb = p1 - p0, nrows = r1 - r0;
-        mbar_wait(full + 8 * s, ph);
+        ring.wait();
         if (nnzb <= SP_NNZ) {
-            const T* vs = reinterpret_cast<const T*>(smem + s * LY::STAGE);
-            const int32_t* cs = reinterpret_cast<const int32_t*>(smem + s * LY::STAGE + LY::VAL_BYTES);
-            const int32_t* rs = reinterpret_cast<const int32_t*>(smem + s * LY::STAGE + LY::VAL_BYTES + LY::COL_BYTES);
+            const uint8_t* const st = ring.stage(ring.s);
+            const T* vs = reinterpret_cast<const T*>(st);
+            const int32_t* cs = reinterpret_cast<const int32_t*>(st + SG::OFF_COL);
+            const int32_t* rs = reinterpret_cast<const int32_t*>(st + SG::OFF_RP);
             const int p0a = p0 & ~3, r0a = r0 & ~3;
             const bool rp_staged = nrows <= SPP_RMAX;
             const int off = p0 - p0a;
@@ -1047,7 +943,7 @@ k_spmm_pipe(const int32_t* __restrict__ rowptr, const int32_t* __restrict__ coli
                 cc[u] = (i < nnzb) ? cs[off + i] : 0;
             }
             for (int iv = 0; iv < np; ++iv) {
-                T* prod = reinterpret_cast<T*>(smem + SpmLayout<T>::OFF_PROD + (iv & 1) * SpmLayout<T>::PROD_BYTES);
+                T* prod = reinterpret_cast<T*>(smem + SpmRing<T>::OFF_EXTRA + (iv & 1) * SG::VAL_BYTES);
                 const T* xi = xcol(iv);
                 T xv[U];
 #pragma unroll
@@ -1089,9 +985,7 @@ k_spmm_pipe(const int32_t* __restrict__ rowptr, const int32_t* __restrict__ coli
                 }
             }
         }
-        __syncwarp();
-        if (lane == 0) mbar_arrive(empty + 8 * s);
-        if (++s == SPM_NSTG) { s = 0; ph ^= 1; }
+        ring.release(false);
     }
 }
 
@@ -2163,20 +2057,20 @@ extern "C" int32_t b2k_debug_apply_fused(b2k_ctx* ctx, const b2k_op* op, b2k_vec
 // opt in to > 48 KB dynamic shared memory for the pipelined SpMV (called per context)
 int32_t b2k_spmv_init(b2k_ctx* ctx) {
     B2K_CUDA(ctx, cudaFuncSetAttribute(k_spmm_pipe<double>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                       SpmLayout<double>::SMEM));
+                                       SpmRing<double>::SMEM));
     B2K_CUDA(ctx, cudaFuncSetAttribute(k_spmm_pipe<float>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                       SpmLayout<float>::SMEM));
+                                       SpmRing<float>::SMEM));
     B2K_CUDA(ctx, cudaFuncSetAttribute((k_spmv_pipe<double, 3, 3>), cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                       SppLayout<double, 3>::SMEM));
+                                       SppRing<double, 3>::SMEM));
     B2K_CUDA(ctx, cudaFuncSetAttribute((k_spmv_pipe<float, 3, 3>), cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                       SppLayout<float, 3>::SMEM));
+                                       SppRing<float, 3>::SMEM));
     B2K_CUDA(ctx, cudaFuncSetAttribute((k_spmv_pipe<double, 2, 4>), cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                       SppLayout<double, 2>::SMEM));
+                                       SppRing<double, 2>::SMEM));
     B2K_CUDA(ctx, cudaFuncSetAttribute((k_spmv_pipe<float, 2, 4>), cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                       SppLayout<float, 2>::SMEM));
+                                       SppRing<float, 2>::SMEM));
 #define SPC_ATTR(T, VS, IS)                                                                                    \
     B2K_CUDA(ctx, cudaFuncSetAttribute((k_spmv_compact<T, VS, IS>), cudaFuncAttributeMaxDynamicSharedMemorySize, \
-                                       SpcLayout<T, VS, IS>::SMEM))
+                                       SpcLayout<T, VS, IS>::Ring::SMEM))
     SPC_ATTR(double, float, int16_t);
     SPC_ATTR(double, float, int32_t);
     SPC_ATTR(double, double, int16_t);
@@ -2185,7 +2079,7 @@ int32_t b2k_spmv_init(b2k_ctx* ctx) {
     if (const char* e = getenv("B2K_CSR_COMPACT")) g_csr_compact = e[0] != '0';
 #define PEN_ATTR(T, MODE)                                                                                      \
     B2K_CUDA(ctx, cudaFuncSetAttribute((k_spmv_pencil<T, PEN_NSTG, PenCtas<T>::N, MODE>),                     \
-                                       cudaFuncAttributeMaxDynamicSharedMemorySize, PenLayout<T, PEN_NSTG>::SMEM))
+                                       cudaFuncAttributeMaxDynamicSharedMemorySize, PenRing<T>::SMEM))
     PEN_ATTR(double, 0);
     PEN_ATTR(double, 1);
     PEN_ATTR(float, 0);
@@ -2341,7 +2235,7 @@ int32_t b2k_enqueue_apply_fused(b2k_ctx* ctx, const b2k_op* op, const VecRef& x,
         g_spmv_launch[0] = 3; g_spmv_launch[2] = grid; g_spmv_launch[3] = op->nblk;
         g_spmv_launch[1] = (ctx->dtype == B2K_F32 || op->cvals ? 1 : 0) | (op->ccol ? 2 : 0);
 #define LAUNCH_C(T, VS, IS, cv, cc)                                                                            \
-    k_spmv_compact<T, VS, IS><<<grid, SPP_THREADS, SpcLayout<T, VS, IS>::SMEM, ctx->stream>>>(                 \
+    k_spmv_compact<T, VS, IS><<<grid, SPP_THREADS, SpcLayout<T, VS, IS>::Ring::SMEM, ctx->stream>>>(                 \
         op->rowptr, op->colidx, (const T*)op->vals, (const VS*)(cv), (const IS*)(cc), op->crp, (const T*)xsrc, \
         (T*)y.ptr, op->rowblk, op->pblk, op->nblk, (T)a0, (T)a1, shifted ? 1 : 0, (const T*)x.ptr,            \
         dotv ? (const T*)dotv->ptr : nullptr, op->part, ctx->d_sync, out, fz)
@@ -2358,7 +2252,7 @@ int32_t b2k_enqueue_apply_fused(b2k_ctx* ctx, const b2k_op* op, const VecRef& x,
         const int grid = std::min(op->nblk, per_sm * ctx->num_sms);
         g_spmv_launch[0] = 2; g_spmv_launch[1] = g_spmv_variant; g_spmv_launch[2] = grid; g_spmv_launch[3] = op->nblk;
 #define LAUNCH_V(T, NS, MB)                                                                    \
-    k_spmv_pipe<T, NS, MB><<<grid, SPP_THREADS, SppLayout<T, NS>::SMEM, ctx->stream>>>(        \
+    k_spmv_pipe<T, NS, MB><<<grid, SPP_THREADS, SppRing<T, NS>::SMEM, ctx->stream>>>(        \
         op->rowptr, op->colidx, (const T*)op->vals, (const T*)xsrc, (const T*)halo, n_loc,     \
         (T*)y.ptr, op->rowblk, op->pblk, op->nblk, (T)a0, (T)a1, shifted ? 1 : 0,              \
         (const T*)x.ptr, dotv ? (const T*)dotv->ptr : nullptr, op->part, ctx->d_sync, out, fz, ps)
@@ -2525,7 +2419,7 @@ static int32_t pencil_launch(b2k_ctx* ctx, const b2k_pencil* P, const VecRef& x,
     const b2k_op* A = P->A;
     const int grid = std::min(A->nblk, PenCtas<T>::N * ctx->num_sms);
     const int pr = b2k_prof_begin(ctx, 0, bytes);
-    k_spmv_pencil<T, PEN_NSTG, PenCtas<T>::N, MODE><<<grid, SPP_THREADS, PenLayout<T, PEN_NSTG>::SMEM, ctx->stream>>>(
+    k_spmv_pencil<T, PEN_NSTG, PenCtas<T>::N, MODE><<<grid, SPP_THREADS, PenRing<T>::SMEM, ctx->stream>>>(
         A->rowptr, A->colidx, (const T*)A->vals, (const T*)P->B->vals, (const T*)x.ptr, (T*)y0.ptr, (T*)y1.ptr,
         A->rowblk, A->pblk, A->nblk, (T)(-rho), vprev ? (const T*)vprev->ptr : nullptr, (T)(-beta), want_dot ? 1 : 0,
         g_pencil_l2_hints ? 1 : 0, ctx->d_part_s, ctx->d_sync, ctx->d_res);
@@ -2770,11 +2664,11 @@ extern "C" int32_t b2k_op_apply_block(b2k_ctx* ctx, const b2k_op* op, const b2k_
         const int pr = b2k_prof_begin(ctx, 7, (double)op->nnz * (ctx->esize + 4) + 4.0 * (op->n_rows + 1) +
                                                   2.0 * np * ctx->esize * op->n_rows);
         if (ctx->dtype == B2K_F64)
-            k_spmm_pipe<double><<<grid, SPP_THREADS, SpmLayout<double>::SMEM, ctx->stream>>>(
+            k_spmm_pipe<double><<<grid, SPP_THREADS, SpmRing<double>::SMEM, ctx->stream>>>(
                 op->rowptr, op->colidx, (const double*)op->vals, (double*)sp.base, sp.ld, cols, np, op->rowblk,
                 op->pblk, op->nblk);
         else
-            k_spmm_pipe<float><<<grid, SPP_THREADS, SpmLayout<float>::SMEM, ctx->stream>>>(
+            k_spmm_pipe<float><<<grid, SPP_THREADS, SpmRing<float>::SMEM, ctx->stream>>>(
                 op->rowptr, op->colidx, (const float*)op->vals, (float*)sp.base, sp.ld, cols, np, op->rowblk,
                 op->pblk, op->nblk);
         b2k_prof_end(ctx, pr);

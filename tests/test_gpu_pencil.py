@@ -4,8 +4,9 @@ k_spmv_pencil, in Float32 and Float64.
 ax, bx and w are compared bit for bit with the composition of existing calls (b2k_op_apply with A and B, then
 b2k_vec_axpby) and with a host restatement: products rounded in T and summed in CSR order in T; a row longer than the
 1536-nonzero tile as a double sum in the kernel's thread / warp order, rounded once; then w = fma(-ρ, bx, ax) and
-w = fma(-β, vprev, w) with libm's fma (a gcc-built helper, as in test_gpu_blas1.py).  The dots are checked exactly on
-small integers and within the Higham bound of b2k_vec_inner.  Shapes: sizes 1 and 255-257, one tile exactly full, rows
+w = fma(-β, vprev, w) with libm's fma (a gcc-built helper, as in test_gpu_blas1.py).  The dots are checked bit for bit
+with spmv_restate's k_spmv_pipe order at the pencil's grid, exactly on small integers and within the Higham bound of
+b2k_vec_inner.  Shapes: sizes 1 and 255-257, one tile exactly full, rows
 straddling tiles, a long row, and an odd size of millions of rows derived from the SM count.
 """
 import ctypes as C
@@ -20,6 +21,8 @@ pytestmark = pytest.mark.gpu
 
 import krylovkit_jl_b200 as kk
 from krylovkit_jl_b200 import _lib as L
+
+import spmv_restate as R
 
 f64, f32 = np.float64, np.float32
 SP_NNZ = 1536
@@ -207,6 +210,52 @@ def test_apply_and_rayleigh_bitwise(fma, dt, name):
             exact = float(np.dot(x.astype(np.float64), y.astype(np.float64)))
             bound = 2 * n * np.finfo(dt).eps * float(np.dot(np.abs(x).astype(np.float64), np.abs(y).astype(np.float64)))
             assert abs(d - exact) <= bound + 1e-300
+        P.free()
+    finally:
+        ctx.close()
+
+
+def device_tiles(op):
+    lib, nblk = L.load(), C.c_int32()
+    assert lib.b2k_debug_op_tiles(op.ctx.h, op.h, None, C.byref(nblk)) == L.OK
+    rb = np.empty(nblk.value + 1, dtype=np.int32)
+    assert lib.b2k_debug_op_tiles(op.ctx.h, op.h, rb.ctypes.data_as(C.POINTER(C.c_int32)), C.byref(nblk)) == L.OK
+    return rb.astype(np.int64)
+
+
+@pytest.mark.parametrize("dt", [f64, f32])
+@pytest.mark.parametrize("name", SHAPES)
+def test_dots_bitwise(fma, dt, name):
+    """<x, w> (MODE 0, with and without vprev), <x, Ax> and <x, Bx> (MODE 1) bit for bit with k_spmv_pipe's dot order
+    at the pencil's grid (3 CTAs per SM in Float64, 4 in Float32): per consumer thread an fma chain in T over its rows,
+    the CTA's warps in order, the last CTA adding the partials in CTA order"""
+    rng = np.random.default_rng(zlib.crc32(f"dots-{name}-{np.dtype(dt).name}".encode()))
+    Pat = shape(name, rng)
+    n = Pat.shape[0]
+    A, B = with_values(Pat, rng, dt)
+    ctx = kk.B200Context(n, 16, dtype=dt)
+    try:
+        dA, dB = upload(ctx, A), upload(ctx, B)
+        P = kk.B200Pencil(dA, dB)
+        x = rng.standard_normal(n).astype(dt)
+        vp = rng.standard_normal(n).astype(dt)
+        xd, vpd = ctx.from_host(x), ctx.from_host(vp)
+        rowblk = device_tiles(dA)
+        grid = min(len(rowblk) - 1, (3 if dt == f64 else 4) * num_sms())
+        gid, rank = R.csr_threads(rowblk, grid)
+        ax_ref, bx_ref = spmv_restated(A, x, dt), spmv_restated(B, x, dt)
+        for use_prev in (False, True):
+            w, bx = ctx.empty(), ctx.empty()
+            dot = P.apply_into(xd, w, bx, 0.37, vpd if use_prev else None, 0.61, dot=True)
+            wref = fma(-0.37, bx_ref, ax_ref, dt)
+            if use_prev:
+                wref = fma(-0.61, vp, wref, dt)
+            np.testing.assert_array_equal(w.to_host(), wref)
+            assert dot == R.dot(fma, dt, x, wref, gid, rank, grid, "pipe"), use_prev
+        ax, bx = ctx.empty(), ctx.empty()
+        xax, xbx = P.rayleigh_into(xd, ax, bx)
+        assert xax == R.dot(fma, dt, x, ax_ref, gid, rank, grid, "pipe")
+        assert xbx == R.dot(fma, dt, x, bx_ref, gid, rank, grid, "pipe")
         P.free()
     finally:
         ctx.close()
