@@ -16,6 +16,9 @@ the order the kernels use:
              Each CTA reduces its threads (pipe / compact: butterflies, then the warps in order; stream / stencil:
              block_sum); the last CTA has thread t add partials t, t + 256, ... from 0.0 and reduces those the same way.
 The grid G is the one the device reports (b2k_debug_spmv_launch).
+k_spmm_pipe (apply to a block, test_gpu_spmm.py) forms every row of every vector as k_spmv_pipe does without xscale:
+csr_rows(..., xscale=None, kernel="pipe").  Its long row is the same strided double sums, warp_sum butterflies and
+red[0 .. 7] added in order from 0.0 by thread 0, so it needs no variant of its own.
 """
 import numpy as np
 
@@ -84,13 +87,16 @@ def last_cta(part, kernel):
 
 
 def row_sums(rowptr, prod, dt):
-    """each row's rounded products summed from (T)0 in stored order (rows of any length)"""
+    """each row's rounded products summed from (T)0 in stored order (rows of any length); step k touches only the
+    rows longer than k, so the work is O(nnz) whatever the longest row"""
     rowptr = np.asarray(rowptr, dtype=np.int64)
     lens = np.diff(rowptr)
     s = np.zeros(len(lens), dtype=dt)
-    for k in range(int(lens.max(initial=0))):
-        m = lens > k
-        s[m] = s[m] + prod[rowptr[:-1][m] + k]
+    rows, k = np.flatnonzero(lens > 0), 0
+    while rows.size:
+        s[rows] = s[rows] + prod[rowptr[rows] + k]
+        k += 1
+        rows = rows[lens[rows] > k]
     return s
 
 
