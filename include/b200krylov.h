@@ -361,6 +361,24 @@ int32_t b2k_lanczos_expand_many(b2k_ctx* ctx, const b2k_op* op, b2k_vec* cols, i
                                 int32_t nsteps, double beta_old, double tol, int32_t alg, double eta,
                                 double* alphas_out, double* betas_out, int32_t* steps_done,
                                 b2k_vec* r_out);
+/* Up to `nsteps` (<= B2K_MAX_CHAIN = 512) consecutive GKL expand! steps — src/factorizations/gkl.jl:246-269 with
+ * gklrecurrence :308-323 — for a CSR matrix A (m x n) and its exact transpose At (n x m, b2k_op_create_transpose),
+ * chained on the device with ONE host synchronisation per call: three launches per ClassicalGramSchmidt2 step (At
+ * SpMV, A SpMV, one cooperative Gram-Schmidt sweep over U), one more with ModifiedGramSchmidt2Blocked (the same sweep
+ * over V), and one flush launch per call.  ucols (capacity k + nsteps + 1) holds U in [0, k) and the residual r in
+ * [k]; vcols (capacity k + nsteps) holds V in [0, k).  On return the d = *steps_done new vectors are ucols[k .. k+d)
+ * and vcols[k .. k+d), *r_out (= ucols[k + d]) is the new residual, alphas_out / betas_out hold one entry per step.
+ * HANDLES as b2k_lanczos_expand_many's chained path: the new columns are allocated by the library and the residual
+ * handle passed in is RELEASED when d > 0.  Stops early after a step with beta <= tol or a non-finite alpha or beta
+ * (its beta is reported as NaN when alpha is not finite); the steps enqueued behind it do nothing.  A non-zero status
+ * can come with *steps_done > 0: those steps are valid.  Vectors are rounded exactly like the scale!! / add!! they
+ * replace, given the same scalars; alpha and beta are deterministic per-CTA sums (as b2k_op_apply_dot) and may differ
+ * from b2k_vec_norm in the last bits.  A refused call writes nothing: B2K_ENOTSUP for alg other than CGS2 / MGS2B, a
+ * dense or matrix-free operator, a row-sharded context, or more columns than the sweep's panel ring holds; B2K_EDIM
+ * when At's shape is not A's transposed or a column is not in one space of the right length (U, r: m; V: n). */
+int32_t b2k_gkl_expand_many(b2k_ctx* ctx, const b2k_op* A, const b2k_op* At, b2k_vec* ucols, b2k_vec* vcols,
+                            int32_t k, int32_t nsteps, double beta_old, double tol, int32_t alg,
+                            double* alphas_out, double* betas_out, int32_t* steps_done, b2k_vec* r_out);
 /* basistransform!(b, U): b[j] <- sum_i b[i]*U[i,j], j < keep — src/orthonormal.jl:291-354.
  * U is host column-major m x keep (ldu).  In place on cols[0..keep) (row-tile resident). */
 int32_t b2k_basis_transform(b2k_ctx* ctx, const b2k_vec* cols, int32_t m,

@@ -128,6 +128,9 @@ _PROTOS = {
     "b2k_lanczos_expand_many": (C.c_int32, [c_ctx, c_op, P(c_vec), C.c_int32, C.c_int32, C.c_double,
                                             C.c_double, C.c_int32, C.c_double, P(C.c_double),
                                             P(C.c_double), P(C.c_int32), P(c_vec)]),
+    "b2k_gkl_expand_many": (C.c_int32, [c_ctx, c_op, c_op, P(c_vec), P(c_vec), C.c_int32, C.c_int32, C.c_double,
+                                        C.c_double, C.c_int32, P(C.c_double), P(C.c_double), P(C.c_int32),
+                                        P(c_vec)]),
     "b2k_basis_transform": (C.c_int32, [c_ctx, P(c_vec), C.c_int32, P(C.c_double), C.c_int32,
                                         C.c_int32]),
     "b2k_basis_rank1update": (C.c_int32, [c_ctx, P(c_vec), C.c_int32, c_vec, P(C.c_double),

@@ -13,6 +13,7 @@ int32_t b2k_enqueue_axpy_dev(b2k_ctx* ctx, void* x, const void* q, int s_slot, i
 // spmv.cu
 int32_t b2k_enqueue_apply(b2k_ctx* ctx, const b2k_op* op, const VecRef& x, const VecRef& y,
                           double a0, double a1, bool shifted, const VecRef* dotv, int dot_slot);
+bool b2k_spmv_tma_on();
 
 using namespace tsk;
 
@@ -165,7 +166,7 @@ k_finalize(const double* __restrict__ A, const double* __restrict__ B, const dou
     FinalizeParams f;
     f.A = A; f.B = B; f.N = N; f.G = G; f.stride = stride; f.k = k; f.res = res; f.off = off; f.noff = noff;
     f.rec = nullptr; f.alpha_col = -1; f.tol = 0.0; f.stop = nullptr; f.ticket = nullptr; f.enabled = 1;
-    f.peer = 0; f.G_local = G;
+    f.peer = 0; f.G_local = G; f.stop_nonfinite = 0;
     finalize_block(f, threadIdx.x, sh);
 }
 
@@ -175,6 +176,40 @@ __global__ void k_lanczos_seed(double* rec, double beta, int* stop) {
     rec[3] = 1.0 / beta;
     rec[4] = beta * beta;
     *stop = 0;
+}
+
+// Records of a chained GKL step i (b2k_gkl_expand_many), rec_i = d_steps + B2K_REC (i + 1), rec_{-1} the seed:
+//   [2] beta_i  [3] 1/beta_i  [4] beta_i^2          (the U sweep's finaliser; [0], [1] unused)
+//   [5] alpha_i [6] 1/alpha_i [7] alpha_i^2         (the A' SpMV's norm epilogue, or the V sweep's finaliser at rec + 3)
+// Step i ran and was the last one to run when alpha_i or beta_i is not finite or beta_i <= tol: the flags the kernels
+// raise, read back from the records.
+__device__ __host__ inline bool gkl_step_stops(const double* rec, double tol) {
+    return !isfinite(rec[5]) || !isfinite(rec[2]) || rec[2] <= tol;
+}
+
+struct GklFlush {
+    const double* rec0;
+    double tol;
+    int nsteps;
+    int64_t ld, n;
+    int32_t col[B2K_MAX_CHAIN];     // V column of step i
+};
+
+// The flush launch of a chained GKL batch: the last step that ran leaves its v~ unnormalised (the next step's A'
+// SpMV would have normalised it), so v = rn(v~ * (1/alpha)) here, whether or not the chain stopped early.
+template <typename T>
+__global__ void __launch_bounds__(256) k_gkl_flush(T* base, const __grid_constant__ GklFlush f) {
+    __shared__ int last;
+    if (threadIdx.x == 0) {
+        int i = 0;
+        while (i + 1 < f.nsteps && !gkl_step_stops(f.rec0 + (size_t)B2K_REC * (i + 1), f.tol)) ++i;
+        last = i;
+    }
+    __syncthreads();
+    const T s = (T)f.rec0[(size_t)B2K_REC * (last + 1) + 6];
+    T* v = base + (int64_t)f.col[last] * f.ld;
+    for (int64_t r = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; r < f.n; r += (int64_t)gridDim.x * blockDim.x)
+        v[r] = v[r] * s;
 }
 
 // out[j] = (T) res[j]  (dense adjoint: projection coefficients become a device vector)
@@ -1842,17 +1877,22 @@ bool chain_ok(const b2k_ctx* ctx, const b2k_op* op, const b2k_vec* cols, int32_t
     return (K1 + C - 1) / C <= NS && K1 <= MAXCH * C && K1 <= PEER_SLOT;
 }
 
+// The cooperative CGS sweep of one chained step over the K1 columns of pn, finalised into the device record rec.
+// Lanczos: with the three-term prologue (beta from rec_prev, <v, A v> from rec).  GKL (b2k_gkl_expand_many): no
+// prologue (the SpMV epilogue has subtracted alpha u already), and a non-finite norm raises the stop flag too.
 template <typename T>
 int32_t chain_step_gs(b2k_ctx* ctx, const Panel& pn, int K1, const VecRef& rw, double* rec_prev, double* rec,
-                      double tol, const PeerStep* psp) {
+                      double tol, const PeerStep* psp, bool prologue = true, int stop_nonfinite = 0) {
     const int grid = grid_for_rows<T>(ctx, pn.n);
     ColList cl;
-    lanczos_cols(cl, pn, K1, true);
+    lanczos_cols(cl, pn, K1, prologue);
     double* PA = b2k_part_set(ctx, 0);
     double* PN = b2k_part_set(ctx, 2);
     FusedParams<T> fp;
     // the prologue's beta is the previous step's, <v, A v> this step's (the SpMV wrote it)
-    lanczos_sweeps<T>(ctx, fp, pn, K1, rw, grid, true, 0.0, 0.0, rec_prev + 2, rec + 0);
+    lanczos_sweeps<T>(ctx, fp, pn, K1, rw, grid, prologue, 0.0, 0.0, prologue ? rec_prev + 2 : nullptr,
+                      prologue ? rec + 0 : nullptr);
+    fp.fin.stop_nonfinite = stop_nonfinite;
     fp.stop = reinterpret_cast<const int*>(ctx->d_sync + B2K_SYNC_STOP);
     fp.trace = ctx->d_trace;
     fp.fin.A = PA; fp.fin.B = nullptr; fp.fin.N = PN; fp.fin.G = grid; fp.fin.stride = B2K_KSTRIDE;
@@ -2043,6 +2083,209 @@ extern "C" int32_t b2k_lanczos_expand_many(b2k_ctx* ctx, const b2k_op* op, b2k_v
         if (beta <= tol) break;
     }
     return B2K_OK;
+}
+
+// ---------------------------------------------------------------------------------------
+// Device-chained GKL steps (gkl.jl:246-269 + 308-323, CGS2 / the flagged MGS2B), THREE launches per CGS2 step and no
+// host round trip between steps.  The operators are rectangular, so each SpMV finishes the previous vector of its own
+// row space in its epilogue (SpmvFuse::pvec) instead of storing its normalised operand:
+//   1. A' r (n rows): gathers r * (1/beta) (u_k, xscale); row j: v_{k-1} = rn(v~_{k-1} * (1/alpha_{k-1})) stored in
+//      place, v~_k = fma(-beta, v_{k-1}, y_j); sum v~_k^2 -> alpha, 1/alpha in the step record (CGS2);
+//      MGS2B: the cooperative sweep over V then removes V' v~_k and its finaliser writes alpha instead;
+//   2. A v~_k (m rows): gathers v~_k * (1/alpha) (v_k); row i: u_k = rn(r_i * (1/beta)) stored to its column,
+//      r'_i = fma(-alpha, u_k, y_i);
+//   3. the cooperative CGS sweep of r' over U (chain_step_gs without the Lanczos prologue); its finaliser writes beta,
+//      1/beta and raises the stop flag on beta <= tol or a non-finite beta.
+// A flush launch at the end of the call normalises the v~ of the last step that ran (k_gkl_flush).
+// Rounding: every vector is rounded like the scale!! / add!! it replaces, given the same scalars; alpha and beta are
+// the CTA-ordered sums of the fused dot (b2k_op_apply_dot) and the sweep, which may differ from b2k_vec_norm in the
+// last bits.  A batch of N steps gives the bits of N calls of one step.
+namespace {
+
+int32_t gkl_refuse(b2k_ctx* ctx, const b2k_op* A, const b2k_op* At, const b2k_vec* ucols, const b2k_vec* vcols,
+                   int32_t k, int32_t nsteps, int32_t alg) {
+    if (alg != B2K_CGS2 && alg != B2K_MGS2B)
+        return b2k_fail(ctx, B2K_ENOTSUP, "gkl_expand_many: ClassicalGramSchmidt2 / ModifiedGramSchmidt2Blocked only");
+    if (ctx->nranks > 1) return b2k_fail(ctx, B2K_ENOTSUP, "gkl_expand_many: row-sharded contexts are not supported");
+    int64_t m = 0, n = 0, tm = 0, tn = 0;
+    int32_t ka = -1, kt = -1;
+    B2K_TRY(b2k_op_info(A, &m, &n, nullptr, &ka));
+    B2K_TRY(b2k_op_info(At, &tm, &tn, nullptr, &kt));
+    if (ka != 0 || kt != 0)
+        return b2k_fail(ctx, B2K_ENOTSUP, "gkl_expand_many: A and A' must be stored CSR matrices");
+    if (!g_use_coop || !b2k_spmv_tma_on())
+        return b2k_fail(ctx, B2K_ENOTSUP, "gkl_expand_many: needs the cooperative sweep and the TMA SpMV kernels");
+    if (tm != n || tn != m)
+        return b2k_fail(ctx, B2K_EDIM, "gkl_expand_many: A' is %lld x %lld, A is %lld x %lld", (long long)tm,
+                        (long long)tn, (long long)m, (long long)n);
+    VecRef t;
+    int32_t su = -1, sv = -1;
+    for (int i = 0; i <= k; ++i) {
+        B2K_TRY(b2k_resolve(ctx, ucols[i], &t));
+        if (i == 0) su = t.space;
+        if (t.space != su || t.n != m)
+            return b2k_fail(ctx, B2K_EDIM, "gkl_expand_many: U and r must be columns of one space of length %lld",
+                            (long long)m);
+    }
+    for (int i = 0; i < k; ++i) {
+        B2K_TRY(b2k_resolve(ctx, vcols[i], &t));
+        if (i == 0) sv = t.space;
+        if (t.space != sv || t.n != n)
+            return b2k_fail(ctx, B2K_EDIM, "gkl_expand_many: V must be columns of one space of length %lld",
+                            (long long)n);
+    }
+    const int C = ctx->dtype == B2K_F64 ? 8 : 16;
+    const int K1 = k + nsteps;
+    if ((K1 + C - 1) / C > NS || K1 > MAXCH * C || K1 > 256)
+        return b2k_fail(ctx, B2K_ENOTSUP, "gkl_expand_many: %d columns do not fit the sweep's panel ring", K1);
+    return B2K_OK;
+}
+
+int32_t gkl_chain(b2k_ctx* ctx, const b2k_op* A, const b2k_op* At, b2k_vec* ucols, b2k_vec* vcols, int32_t k,
+                  int32_t nsteps, double beta_old, double tol, int32_t alg, double* alphas_out, double* betas_out,
+                  int32_t* steps_done, b2k_vec* r_out) {
+    const bool f64 = ctx->dtype == B2K_F64;
+    const int32_t su = B2K_VEC_SPACE(ucols[k]), sv = B2K_VEC_SPACE(vcols[0]);
+    double* rec0 = ctx->d_steps;
+    int* d_stop = reinterpret_cast<int*>(ctx->d_sync + B2K_SYNC_STOP);
+    k_lanczos_seed<<<1, 1, 0, ctx->stream>>>(rec0, beta_old, d_stop);
+    B2K_LAUNCH_CHECK(ctx);
+    std::vector<b2k_vec> touched, Uh, Vh, Wh;
+    touched.push_back(ucols[k]);
+    GklFlush fl;
+    memset(&fl, 0, sizeof(fl));
+    int32_t enq = 0, rc = B2K_OK;
+    auto fuse = [&]() {
+        SpmvFuse fz;
+        memset(&fz, 0, sizeof(fz));
+        fz.stop = d_stop;
+        fz.l2_hints = g_l2_hints ? 1 : 0;
+        fz.trace = ctx->d_trace;
+        return fz;
+    };
+    for (int32_t i = 0; i < nsteps; ++i) {
+        const int32_t K = k + i;                 // basis size before this step
+        const b2k_vec R = ucols[K];
+        b2k_vec Vc = -1, Uc = -1, W = -1;
+        if ((rc = b2k_vec_alloc(ctx, sv, &Vc)) != B2K_OK) break;
+        touched.push_back(Vc);
+        if ((rc = b2k_vec_alloc(ctx, su, &Uc)) != B2K_OK) break;
+        touched.push_back(Uc);
+        if ((rc = b2k_vec_alloc(ctx, su, &W)) != B2K_OK) break;
+        touched.push_back(W);
+        VecRef rR, rV, rU, rW, vprev;
+        rc = b2k_resolve(ctx, R, &rR);
+        if (rc == B2K_OK) rc = b2k_resolve(ctx, Vc, &rV);
+        if (rc == B2K_OK) rc = b2k_resolve(ctx, Uc, &rU);
+        if (rc == B2K_OK) rc = b2k_resolve(ctx, W, &rW);
+        if (rc == B2K_OK) rc = b2k_resolve(ctx, vcols[K - 1], &vprev);
+        if (rc != B2K_OK) break;
+        double* rec_prev = rec0 + (size_t)B2K_REC * i;
+        double* rec = rec0 + (size_t)B2K_REC * (i + 1);
+        // 1. v~_k = A' (r / beta) - beta v_{k-1}, finishing v_{k-1} on the way (the caller's V[k-1] is final)
+        SpmvFuse fa = fuse();
+        fa.xscale = rec_prev + 3;
+        fa.pvec = vprev.ptr;
+        if (i > 0) {
+            fa.pscale = rec_prev + 6;
+            fa.pout = vprev.ptr;
+        }
+        fa.acoef = rec_prev + 2;
+        if (alg == B2K_CGS2) fa.nrm_out = rec + 5;
+        if ((rc = b2k_enqueue_apply_fused(ctx, At, rR, rV, 0.0, 1.0, false, nullptr, nullptr, &fa)) != B2K_OK) break;
+        vcols[K] = Vc;
+        if (alg == B2K_MGS2B) {                  // the flagged MGS2B: v~_k -= V V' v~_k, alpha from the finaliser
+            Panel pv;
+            if ((rc = make_panel(ctx, vcols, K, &pv)) != B2K_OK) break;
+            rc = f64 ? chain_step_gs<double>(ctx, pv, K, rV, nullptr, rec + 3, -INFINITY, nullptr, false, 1)
+                     : chain_step_gs<float>(ctx, pv, K, rV, nullptr, rec + 3, -INFINITY, nullptr, false, 1);
+            if (rc != B2K_OK) break;
+        }
+        // 2. r' = A (v~_k / alpha) - alpha u_k, u_k = r / beta stored to its column
+        SpmvFuse fb = fuse();
+        fb.xscale = rec + 6;
+        fb.pvec = rR.ptr;
+        fb.pscale = rec_prev + 3;
+        fb.pout = rU.ptr;
+        fb.acoef = rec + 5;
+        if ((rc = b2k_enqueue_apply_fused(ctx, A, rV, rW, 0.0, 1.0, false, nullptr, nullptr, &fb)) != B2K_OK) break;
+        ucols[K] = Uc;
+        // 3. r' -= U U' r', beta = ||r'||
+        Panel pu;
+        if ((rc = make_panel(ctx, ucols, K + 1, &pu)) != B2K_OK) break;
+        rc = f64 ? chain_step_gs<double>(ctx, pu, K + 1, rW, rec_prev, rec, tol, nullptr, false, 1)
+                 : chain_step_gs<float>(ctx, pu, K + 1, rW, rec_prev, rec, tol, nullptr, false, 1);
+        if (rc != B2K_OK) break;
+        ucols[K + 1] = W;
+        Uh.push_back(Uc);
+        Vh.push_back(Vc);
+        Wh.push_back(W);
+        fl.col[i] = B2K_VEC_COL(Vc);
+        // r's column has been read for the last time; later steps may reuse it (stream order keeps that safe)
+        ctx->spaces[su].used[B2K_VEC_COL(R)] = 0;
+        ++enq;
+    }
+    if (enq > 0) {
+        const B2kSpace& s = ctx->spaces[sv];
+        fl.rec0 = rec0; fl.tol = tol; fl.nsteps = enq; fl.ld = s.ld; fl.n = s.n;
+        const int grid = (int)std::max<int64_t>(1, std::min<int64_t>((s.n + 255) / 256, (int64_t)ctx->num_sms * 4));
+        if (f64) k_gkl_flush<double><<<grid, 256, 0, ctx->stream>>>((double*)s.base, fl);
+        else k_gkl_flush<float><<<grid, 256, 0, ctx->stream>>>((float*)s.base, fl);
+        B2K_LAUNCH_CHECK(ctx);
+    }
+    int32_t d = 0;
+    if (enq > 0) {
+        cudaError_t e = cudaMemcpyAsync(ctx->h_res, rec0 + B2K_REC, sizeof(double) * B2K_REC * enq,
+                                        cudaMemcpyDeviceToHost, ctx->stream);
+        if (e != cudaSuccess) return b2k_fail(ctx, B2K_ECUDA, "gkl_expand_many: %s", cudaGetErrorString(e));
+        B2K_TRY(b2k_stream_sync(ctx));
+        d = enq;
+        for (int32_t i = 0; i < enq; ++i) {
+            const double* r = ctx->h_res + (size_t)B2K_REC * i;
+            alphas_out[i] = r[5];
+            betas_out[i] = isfinite(r[5]) ? r[2] : NAN;     // a non-finite alpha stopped the step before its beta
+            if (gkl_step_stops(r, tol)) { d = i + 1; break; }
+        }
+    } else {
+        cudaStreamSynchronize(ctx->stream);
+    }
+    // column bookkeeping: everything this batch touched is free again, except the d new columns of U and V and the
+    // residual that follows them (steps behind a stop were skipped on the device)
+    for (b2k_vec h : touched) ctx->spaces[B2K_VEC_SPACE(h)].used[B2K_VEC_COL(h)] = 0;
+    if (d > 0) {
+        for (int32_t i = 0; i < d; ++i) {
+            ucols[k + i] = Uh[i];
+            vcols[k + i] = Vh[i];
+            ctx->spaces[su].used[B2K_VEC_COL(Uh[i])] = 1;
+            ctx->spaces[sv].used[B2K_VEC_COL(Vh[i])] = 1;
+        }
+        ucols[k + d] = Wh[d - 1];
+        ctx->spaces[su].used[B2K_VEC_COL(Wh[d - 1])] = 1;
+    } else {
+        ucols[k] = touched[0];                   // nothing ran: r is still r
+        ctx->spaces[su].used[B2K_VEC_COL(touched[0])] = 1;
+    }
+    *steps_done = d;
+    *r_out = ucols[k + d];
+    return rc;
+}
+
+}  // namespace
+
+extern "C" int32_t b2k_gkl_expand_many(b2k_ctx* ctx, const b2k_op* A, const b2k_op* At, b2k_vec* ucols,
+                                       b2k_vec* vcols, int32_t k, int32_t nsteps, double beta_old, double tol,
+                                       int32_t alg, double* alphas_out, double* betas_out, int32_t* steps_done,
+                                       b2k_vec* r_out) {
+    if (!ctx) return B2K_EINVAL;
+    if (!A || !At || !ucols || !vcols || !alphas_out || !betas_out || !steps_done || !r_out)
+        return b2k_fail(ctx, B2K_EINVAL, "gkl_expand_many: null pointer");
+    if (k < 1 || nsteps < 1 || nsteps > B2K_MAX_CHAIN)
+        return b2k_fail(ctx, B2K_EINVAL, "gkl_expand_many: need k >= 1 and 1 <= nsteps <= %d", B2K_MAX_CHAIN);
+    if (!(beta_old > 0.0) || !isfinite(beta_old))
+        return b2k_fail(ctx, B2K_EINVAL, "gkl_expand_many: beta_old must be positive and finite");
+    B2K_TRY(gkl_refuse(ctx, A, At, ucols, vcols, k, nsteps, alg));
+    return gkl_chain(ctx, A, At, ucols, vcols, k, nsteps, beta_old, tol, alg, alphas_out, betas_out, steps_done,
+                     r_out);
 }
 
 extern "C" int32_t b2k_basis_transform(b2k_ctx* ctx, const b2k_vec* cols, int32_t m,

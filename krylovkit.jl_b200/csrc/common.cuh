@@ -203,6 +203,19 @@ struct SpmvFuse {
     // boundary rows under (0: the apply pushes them itself)
     unsigned long long seq_alpha, seq_halo;
     unsigned long long* trace;     // optional event trace (b2k_debug_trace)
+    // The GKL step (basis.cu, b2k_gkl_expand_many): read only by the kernel instances with the GKL row epilogue
+    // (b2k_enqueue_apply_fused picks them when pvec is set).  The operators are rectangular, so instead of vout the
+    // epilogue finishes the previous vector of its OWN row space:
+    //   pvec / pscale / pout : p_r = rn(pvec_r * (*pscale)) (pscale null: p_r = pvec_r), stored to pout (may be null,
+    //                          may alias pvec);
+    //   acoef                : y_r = fma(-(*acoef), p_r, (A x)_r) is stored instead of (A x)_r;
+    //   nrm_out              : sum of y_r^2 (fma chain per thread, CTA partials as the fused dot): the last CTA writes
+    //                          {sqrt(s), 1/sqrt(s), s} and raises *stop when sqrt(s) is not finite.
+    const void* pvec;
+    const double* pscale;
+    void* pout;
+    const double* acoef;
+    double* nrm_out;
 };
 
 int32_t b2k_enqueue_apply(b2k_ctx* ctx, const b2k_op* op, const VecRef& x, const VecRef& y,

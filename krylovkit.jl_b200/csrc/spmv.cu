@@ -381,6 +381,19 @@ __device__ __forceinline__ void consumer_sums(const double (&v)[NRED], double* _
     }
 }
 
+// The GKL epilogue's norm (SpmvFuse::nrm_out): the CTA-ordered sum of the threads' y_r^2 chains, as the fused dot; the
+// last CTA stores {sqrt(s), 1/sqrt(s), s} and raises the chain's stop flag when the norm is not finite.
+__device__ __forceinline__ void gkl_norm_sums(double v, double* __restrict__ part, unsigned* __restrict__ ticket,
+                                              double* red, int* flag, const SpmvFuse& fz) {
+    consumer_sums<1>({v}, part, ticket, red, flag, [&](int, double tot) {
+        const double a = sqrt(tot);
+        fz.nrm_out[0] = a;
+        fz.nrm_out[1] = 1.0 / a;
+        fz.nrm_out[2] = tot;
+        if (fz.stop && !isfinite(a)) *const_cast<int*>(fz.stop) = 1;
+    });
+}
+
 __global__ void k_pblk(const int32_t* __restrict__ rowptr, const int32_t* __restrict__ rowblk, int count,
                        int32_t* __restrict__ pblk) {
     const int b = blockIdx.x * blockDim.x + threadIdx.x;
@@ -391,9 +404,12 @@ __global__ void k_pblk(const int32_t* __restrict__ rowptr, const int32_t* __rest
 // shift acting on the normalised operand, vout_r = the normalised x_r, and the dot chain dacc = fma(dv_r, y_r - dsc
 // dsub_r, dacc) over the thread's rows, dv = dotv or the normalised x (fz.dot_self).  load(r) issues a row's global
 // loads, before its sum so that they overlap it; row(r, loads, sum) finishes it.
-template <typename T>
+// GK (the instances b2k_gkl_expand_many launches): after the sum, p_r = rn(pvec_r * pscale) is stored to pout,
+// y_r = fma(-acoef, p_r, sum) is stored instead of the sum, and nacc = fma(y_r, y_r, nacc) when nrm_out is set
+// (SpmvFuse).  Off, none of it is compiled.
+template <typename T, bool GK = false>
 struct RowEpilogue {
-    struct Loads { T dv, xself, xsr, dsv; };
+    struct Loads { T dv, xself, xsr, dsv, pv; };
     const SpmvFuse fz;
     const T* x;
     T* y;
@@ -410,12 +426,30 @@ struct RowEpilogue {
     const T* dsub = reinterpret_cast<const T*>(fz.dot_sub_vec);
     T dsc = dsub ? (T)(*fz.dot_sub_scale) : (T)0;
     T dacc = (T)0;
+    const T* pvec = GK ? reinterpret_cast<const T*>(fz.pvec) : nullptr;
+    T* pout = GK ? reinterpret_cast<T*>(fz.pout) : nullptr;
+    bool pscaled = GK && fz.pscale != nullptr;
+    T psc = pscaled ? (T)(*fz.pscale) : (T)1;
+    T nac = GK ? -(T)(*fz.acoef) : (T)0;
+    bool want_nrm = GK && fz.nrm_out != nullptr;
 
     __device__ __forceinline__ Loads load(int r) const {
         return {(dotv && !fz.dot_self) ? __ldg(dotv + r) : (T)0, self ? __ldg(x + r) : (T)0,
-                shifted ? __ldg(xs + r) : (T)0, dsub ? __ldg(dsub + r) : (T)0};
+                shifted ? __ldg(xs + r) : (T)0, dsub ? __ldg(dsub + r) : (T)0, GK ? pvec[r] : (T)0};
+    }
+    // the GKL step's finish of row r: the previous vector normalised and stored, the axpy, the norm chain
+    __device__ __forceinline__ T gkl_row(int r, T pv, T sum) {
+        const T p = pscaled ? mul_rn<T>(pv, psc) : pv;
+        if (pout) pout[r] = p;
+        sum = fma(nac, p, sum);
+        if (want_nrm) dacc = fma(sum, sum, dacc);
+        return sum;
     }
     __device__ __forceinline__ void row(int r, const Loads& l, T sum) {
+        if constexpr (GK) {
+            y[r] = gkl_row(r, l.pv, sum);
+            return;
+        }
         if (shifted) sum = fma(a0, l.xsr * sc, a1 * sum);      // the shift acts on the normalised operand
         if (fz.l2_hints) st_hint(y + r, sum, pol_last);
         else y[r] = sum;
@@ -446,15 +480,19 @@ struct RowEpilogue {
             double tot = 0.0;
             for (int i = 0; i < SPP_CONS / 32; ++i) tot += red[i];
             T sum = (T)tot;
-            if (shifted) sum = fma(a0, xs[r0] * sc, a1 * sum);
-            y[r0] = sum;
-            T dv = (dotv && !fz.dot_self) ? dotv[r0] : (T)0;
-            if (self) {
-                const T vn = __ldg(x + r0) * sc;
-                if (vout) vout[r0] = vn;
-                if (fz.dot_self) dv = vn;
+            if constexpr (GK) {
+                y[r0] = gkl_row(r0, pvec[r0], sum);
+            } else {
+                if (shifted) sum = fma(a0, xs[r0] * sc, a1 * sum);
+                y[r0] = sum;
+                T dv = (dotv && !fz.dot_self) ? dotv[r0] : (T)0;
+                if (self) {
+                    const T vn = __ldg(x + r0) * sc;
+                    if (vout) vout[r0] = vn;
+                    if (fz.dot_self) dv = vn;
+                }
+                if (want_dot) dacc = fma(dv, dsub ? fma(-dsc, dsub[r0], sum) : sum, dacc);
             }
-            if (want_dot) dacc = fma(dv, dsub ? fma(-dsc, dsub[r0], sum) : sum, dacc);
         }
         named_bar_sync(1, SPP_CONS);
     }
@@ -462,7 +500,7 @@ struct RowEpilogue {
 
 // NSTG ring stages, MINB CTAs per SM (variants: (3, 3); (2, 4): fewer stages, more resident warps to hide the
 // latency of the x gather)
-template <typename T, int NSTG, int MINB>
+template <typename T, int NSTG, int MINB, bool GK = false>
 __global__ void __launch_bounds__(SPP_THREADS, MINB)
 k_spmv_pipe(const int32_t* __restrict__ rowptr, const int32_t* __restrict__ colidx,
             const T* __restrict__ vals, const T* __restrict__ x, const T* __restrict__ halo,
@@ -494,7 +532,7 @@ k_spmv_pipe(const int32_t* __restrict__ rowptr, const int32_t* __restrict__ coli
         named_bar_sync(1, SPP_CONS);
     }
     if (tr0) b2k_trace(fz.trace, 2);
-    RowEpilogue<T> ep{fz, x, y, xs, dotv, a0, a1, shifted};
+    RowEpilogue<T, GK> ep{fz, x, y, xs, dotv, a0, a1, shifted};
     ring.start();
     for (int tile = blockIdx.x; tile < nblk; tile += gridDim.x) {
         const int4 d = ring.next(tile);
@@ -545,7 +583,9 @@ k_spmv_pipe(const int32_t* __restrict__ rowptr, const int32_t* __restrict__ coli
         ring.release();
     }
     if (tr0) b2k_trace(fz.trace, 3);
-    if (ep.want_dot) {
+    if constexpr (GK) {
+        if (ep.want_nrm) gkl_norm_sums((double)ep.dacc, part, ticket, ring.red(), ring.flag(), fz);
+    } else if (ep.want_dot) {
         consumer_sums<1>({(double)ep.dacc}, part, ticket, ring.red(), ring.flag(), [&](int, double tot) {
             *out = tot;
             if (ps.on && ps.seq_alpha) peer_publish1(ps.pd, PEER_CH_ALPHA, ps.seq_alpha, tot);
@@ -585,7 +625,7 @@ template <typename T, typename VS, typename IS> struct SpcLayout {
     static_assert(VAL_BYTES % 16 == 0 && COL_BYTES % 16 == 0 && RP_BYTES % 16 == 0, "TMA needs 16-byte offsets");
 };
 
-template <typename T, typename VS, typename IS>
+template <typename T, typename VS, typename IS, bool GK = false>
 __global__ void __launch_bounds__(SPP_THREADS, SPC_CTAS)
 k_spmv_compact(const int32_t* __restrict__ rowptr, const int32_t* __restrict__ colidx, const T* __restrict__ vals,
                const VS* __restrict__ cvals, const IS* __restrict__ ccol, const uint16_t* __restrict__ crp,
@@ -617,7 +657,7 @@ k_spmv_compact(const int32_t* __restrict__ rowptr, const int32_t* __restrict__ c
     const bool tr0 = fz.trace && blockIdx.x == 0 && tid == 0;
     if (tr0) b2k_trace(fz.trace, 1);
     if (tr0) b2k_trace(fz.trace, 2);
-    RowEpilogue<T> ep{fz, x, y, xs, dotv, a0, a1, shifted};
+    RowEpilogue<T, GK> ep{fz, x, y, xs, dotv, a0, a1, shifted};
     // The x gather of the next tile is issued before the row sums of this one, so its latency (the first touch of an
     // entry of x misses L2) overlaps them instead of stalling the CTA once per tile.
     constexpr int U = SP_NNZ / SPP_CONS;
@@ -692,7 +732,9 @@ k_spmv_compact(const int32_t* __restrict__ rowptr, const int32_t* __restrict__ c
         ring.release();
     }
     if (tr0) b2k_trace(fz.trace, 3);
-    if (ep.want_dot) {
+    if constexpr (GK) {
+        if (ep.want_nrm) gkl_norm_sums((double)ep.dacc, part, ticket, ring.red(), ring.flag(), fz);
+    } else if (ep.want_dot) {
         consumer_sums<1>({(double)ep.dacc}, part, ticket, ring.red(), ring.flag(), [&](int, double tot) {
             *out = tot;
             if (fz.trace) b2k_trace(fz.trace, 4);
@@ -1963,6 +2005,9 @@ extern "C" int32_t b2k_debug_set_spmv_pipe(int32_t on) {
     return B2K_OK;
 }
 
+// is the SpMV of this process one of the TMA kernels (the ones that carry the GKL epilogue)?
+bool b2k_spmv_tma_on() { return g_spmv_pipe; }
+
 extern "C" int32_t b2k_debug_set_spmv_variant(int32_t v) {
     g_spmv_variant = v == 0 ? 0 : 1;
     return B2K_OK;
@@ -2060,17 +2105,22 @@ int32_t b2k_spmv_init(b2k_ctx* ctx) {
                                        SpmRing<double>::SMEM));
     B2K_CUDA(ctx, cudaFuncSetAttribute(k_spmm_pipe<float>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                        SpmRing<float>::SMEM));
-    B2K_CUDA(ctx, cudaFuncSetAttribute((k_spmv_pipe<double, 3, 3>), cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                       SppRing<double, 3>::SMEM));
-    B2K_CUDA(ctx, cudaFuncSetAttribute((k_spmv_pipe<float, 3, 3>), cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                       SppRing<float, 3>::SMEM));
-    B2K_CUDA(ctx, cudaFuncSetAttribute((k_spmv_pipe<double, 2, 4>), cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                       SppRing<double, 2>::SMEM));
-    B2K_CUDA(ctx, cudaFuncSetAttribute((k_spmv_pipe<float, 2, 4>), cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                       SppRing<float, 2>::SMEM));
+    // every instance, with and without the GKL epilogue
+#define SPP_ATTR(T, NS, MB)                                                                                    \
+    B2K_CUDA(ctx, cudaFuncSetAttribute((k_spmv_pipe<T, NS, MB>), cudaFuncAttributeMaxDynamicSharedMemorySize,   \
+                                       SppRing<T, NS>::SMEM));                                                 \
+    B2K_CUDA(ctx, cudaFuncSetAttribute((k_spmv_pipe<T, NS, MB, true>), cudaFuncAttributeMaxDynamicSharedMemorySize, \
+                                       SppRing<T, NS>::SMEM))
+    SPP_ATTR(double, 3, 3);
+    SPP_ATTR(float, 3, 3);
+    SPP_ATTR(double, 2, 4);
+    SPP_ATTR(float, 2, 4);
+#undef SPP_ATTR
 #define SPC_ATTR(T, VS, IS)                                                                                    \
     B2K_CUDA(ctx, cudaFuncSetAttribute((k_spmv_compact<T, VS, IS>), cudaFuncAttributeMaxDynamicSharedMemorySize, \
-                                       SpcLayout<T, VS, IS>::Ring::SMEM))
+                                       SpcLayout<T, VS, IS>::Ring::SMEM));                                     \
+    B2K_CUDA(ctx, cudaFuncSetAttribute((k_spmv_compact<T, VS, IS, true>),                                      \
+                                       cudaFuncAttributeMaxDynamicSharedMemorySize, SpcLayout<T, VS, IS>::Ring::SMEM))
     SPC_ATTR(double, float, int16_t);
     SPC_ATTR(double, float, int32_t);
     SPC_ATTR(double, double, int16_t);
@@ -2125,6 +2175,9 @@ int32_t b2k_enqueue_apply_fused(b2k_ctx* ctx, const b2k_op* op, const VecRef& x,
     if (fzp && op->kind == 1) return b2k_fail(ctx, B2K_ENOTSUP, "fused apply: CSR / stencil operators only");
     if ((fz.vout || fz.dot_self) && (op->n_rows != x.n))
         return b2k_fail(ctx, B2K_EDIM, "fused apply: needs a square operator (row r <-> x[r])");
+    const bool gk = fz.pvec != nullptr;
+    if (gk && (op->kind != 0 || !g_spmv_pipe || ctx->nranks > 1 || !fz.acoef || fz.vout || fz.dot_self || dotv || shifted))
+        return b2k_fail(ctx, B2K_ENOTSUP, "fused apply: the GKL epilogue needs a single-GPU CSR operator and a TMA kernel");
     if (fz.dot_self && !dot_out) return b2k_fail(ctx, B2K_EINVAL, "fused apply: dot_self without an output slot");
     if (op->kind == 1) {
         if (shifted || dotv) return b2k_fail(ctx, B2K_ENOTSUP, "dense apply: no shift/dot fusion");
@@ -2222,11 +2275,12 @@ int32_t b2k_enqueue_apply_fused(b2k_ctx* ctx, const b2k_op* op, const VecRef& x,
         return B2K_OK;
     }
     // algorithmic bytes: matrix (as streamed) + x + y, plus the normalised copy of x a chained Lanczos step stores
-    // (fz.vout)
+    // (fz.vout), or the previous vector the GKL epilogue reads and stores (fz.pvec, fz.pout)
     const bool compact = g_spmv_pipe && g_csr_compact && op->crp != nullptr;
     const double vbytes = (compact && op->cvals) ? 4.0 : (double)ctx->esize, cbytes = (compact && op->ccol) ? 2.0 : 4.0;
     const int pr = b2k_prof_begin(ctx, 0, (double)op->nnz * (vbytes + cbytes) + (compact ? 2.0 : 4.0) * (op->n_rows + 1) +
-                                              (fz.vout ? 3.0 : 2.0) * ctx->esize * op->n_rows);
+                                              (2.0 + (fz.vout ? 1.0 : 0.0) + (gk ? 1.0 : 0.0) + (fz.pout ? 1.0 : 0.0)) *
+                                                  ctx->esize * op->n_rows);
     g_spmv_kernel = compact ? 3 : (g_spmv_pipe ? 2 : 1);
     if (compact) {
         // the grid of k_spmv_pipe's variant: the CTA partials of the dot, and so its rounding, stay the same
@@ -2234,11 +2288,16 @@ int32_t b2k_enqueue_apply_fused(b2k_ctx* ctx, const b2k_op* op, const VecRef& x,
         const int grid = std::min(op->nblk, per_sm * ctx->num_sms);
         g_spmv_launch[0] = 3; g_spmv_launch[2] = grid; g_spmv_launch[3] = op->nblk;
         g_spmv_launch[1] = (ctx->dtype == B2K_F32 || op->cvals ? 1 : 0) | (op->ccol ? 2 : 0);
-#define LAUNCH_C(T, VS, IS, cv, cc)                                                                            \
-    k_spmv_compact<T, VS, IS><<<grid, SPP_THREADS, SpcLayout<T, VS, IS>::Ring::SMEM, ctx->stream>>>(                 \
+#define LAUNCH_CG(T, VS, IS, GK, cv, cc)                                                                       \
+    k_spmv_compact<T, VS, IS, GK><<<grid, SPP_THREADS, SpcLayout<T, VS, IS>::Ring::SMEM, ctx->stream>>>(             \
         op->rowptr, op->colidx, (const T*)op->vals, (const VS*)(cv), (const IS*)(cc), op->crp, (const T*)xsrc, \
         (T*)y.ptr, op->rowblk, op->pblk, op->nblk, (T)a0, (T)a1, shifted ? 1 : 0, (const T*)x.ptr,            \
         dotv ? (const T*)dotv->ptr : nullptr, op->part, ctx->d_sync, out, fz)
+#define LAUNCH_C(T, VS, IS, cv, cc)                                                                            \
+    do {                                                                                                       \
+        if (gk) LAUNCH_CG(T, VS, IS, true, cv, cc);                                                            \
+        else LAUNCH_CG(T, VS, IS, false, cv, cc);                                                              \
+    } while (0)
         if (ctx->dtype == B2K_F64) {
             if (op->cvals && op->ccol) LAUNCH_C(double, float, int16_t, op->cvals, op->ccol);
             else if (op->cvals) LAUNCH_C(double, float, int32_t, op->cvals, op->colidx);
@@ -2247,15 +2306,21 @@ int32_t b2k_enqueue_apply_fused(b2k_ctx* ctx, const b2k_op* op, const VecRef& x,
             LAUNCH_C(float, float, int16_t, op->vals, op->ccol);
         }
 #undef LAUNCH_C
+#undef LAUNCH_CG
     } else if (g_spmv_pipe) {
         const int per_sm = g_spmv_variant == 1 ? 4 : 3;
         const int grid = std::min(op->nblk, per_sm * ctx->num_sms);
         g_spmv_launch[0] = 2; g_spmv_launch[1] = g_spmv_variant; g_spmv_launch[2] = grid; g_spmv_launch[3] = op->nblk;
-#define LAUNCH_V(T, NS, MB)                                                                    \
-    k_spmv_pipe<T, NS, MB><<<grid, SPP_THREADS, SppRing<T, NS>::SMEM, ctx->stream>>>(        \
+#define LAUNCH_VG(T, NS, MB, GK)                                                               \
+    k_spmv_pipe<T, NS, MB, GK><<<grid, SPP_THREADS, SppRing<T, NS>::SMEM, ctx->stream>>>(    \
         op->rowptr, op->colidx, (const T*)op->vals, (const T*)xsrc, (const T*)halo, n_loc,     \
         (T*)y.ptr, op->rowblk, op->pblk, op->nblk, (T)a0, (T)a1, shifted ? 1 : 0,              \
         (const T*)x.ptr, dotv ? (const T*)dotv->ptr : nullptr, op->part, ctx->d_sync, out, fz, ps)
+#define LAUNCH_V(T, NS, MB)                                                                    \
+    do {                                                                                       \
+        if (gk) LAUNCH_VG(T, NS, MB, true);                                                    \
+        else LAUNCH_VG(T, NS, MB, false);                                                      \
+    } while (0)
         if (g_spmv_variant == 1) {
             if (ctx->dtype == B2K_F64) LAUNCH_V(double, 2, 4);
             else LAUNCH_V(float, 2, 4);
@@ -2264,6 +2329,7 @@ int32_t b2k_enqueue_apply_fused(b2k_ctx* ctx, const b2k_op* op, const VecRef& x,
             else LAUNCH_V(float, 3, 3);
         }
 #undef LAUNCH_V
+#undef LAUNCH_VG
     } else {
         g_spmv_launch[0] = 1; g_spmv_launch[1] = 0; g_spmv_launch[2] = op->nblk; g_spmv_launch[3] = op->nblk;
 #define LAUNCH(T)                                                                              \

@@ -468,7 +468,8 @@ __device__ __forceinline__ void consumer_phase(const PhaseParams<T>& p, const Sm
 // the step land in a device record the NEXT step's kernels read — the host never has to be in the loop:
 //   rec[0] = <v, A v> (written by the SpMV)      rec[1] = alpha = rec[0] + h[alpha_col]   (lanczos.jl:321)
 //   rec[2] = beta = sqrt(||w||^2)                 rec[3] = 1/beta                           rec[4] = ||w||^2
-// and *stop = 1 if beta <= tol (the steps already enqueued behind this one then do nothing).
+// and *stop = 1 if beta <= tol, or (stop_nonfinite) beta is not finite (the steps already enqueued behind this one
+// then do nothing).
 struct FinalizeParams {
     const double* A;
     const double* B;
@@ -487,6 +488,7 @@ struct FinalizeParams {
     // over ranks here
     int peer;
     int G_local;
+    int stop_nonfinite;
 };
 
 // `sh` : >= 2 doubles of shared memory; `barrier_id` : named barrier the NCONS calling threads may use
@@ -538,7 +540,7 @@ __device__ __forceinline__ void finalize_block(const FinalizeParams& f, int tid,
             f.rec[2] = beta;
             f.rec[3] = 1.0 / beta;
             f.rec[4] = n2;
-            if (f.stop && beta <= f.tol) *f.stop = 1;
+            if (f.stop && (beta <= f.tol || (f.stop_nonfinite && !isfinite(beta)))) *f.stop = 1;
         }
     }
 }

@@ -25,6 +25,7 @@ like the reference.  One pass where it is safe, two where it is not; `passes` co
 from the two-pass step by rounding at the level of the tolerance asked for (tools/onepass_gkl_study.py, DESIGN.md §6)."""
 from __future__ import annotations
 
+import ctypes as C
 import math
 
 import numpy as np
@@ -35,12 +36,16 @@ from ..operators import B200Dense, apply_adjoint, apply_normal, apply_normal_gra
 from ..orthonormal import OrthonormalBasis, orthogonalize_, unproject_
 from ..vectors import B200Vec
 
+# columns the cooperative Gram-Schmidt sweep of a chained step holds (U and the new residual after the last step):
+# its panel ring, include/b200krylov.h b2k_gkl_expand_many
+CHAIN_COLS = {8: 96, 4: 192}       # by element size: Float64, Float32
+
 
 class GKLIterator:
     """GKLIterator(f, u₀, orth, keepvecs) — gkl.jl:123-139.  u₀ lives in the codomain."""
 
     def __init__(self, operator, u0: B200Vec, orth: Orthogonalizer, keepvecs: bool = True, onepass: bool = False,
-                 onepass_eta: float = 4.0, onepass_eta_tol: float = 0.0):
+                 onepass_eta: float = 4.0, onepass_eta_tol: float = 0.0, pair=None):
         if not keepvecs and (orth.is_reorth2 or orth.is_ir):
             raise ValueError("Cannot use reorthogonalization without keeping all Krylov vectors")
         if onepass and not isinstance(operator, B200Dense):
@@ -51,6 +56,9 @@ class GKLIterator:
         # largest error estimate a recycled A'u may carry (module doc): onepass_eta roundings of a direct product, or
         # an absolute error onepass_eta_tol * eps (= a fraction of the caller's tolerance), whichever is larger
         self.onepass_eta, self.onepass_eta_tol = float(onepass_eta), float(onepass_eta_tol)
+        # (A, A') as B200CSR operators, A' the exact device transpose of A: expand_many_ may chain the steps on the
+        # device (b2k_gkl_expand_many).  A user's (A, At) tuple is not known to be an exact transpose: None.
+        self.pair = pair
 
     def eta_max(self, anorm: float) -> float:
         return max(self.onepass_eta, self.onepass_eta_tol / anorm if anorm > 0 else 0.0)
@@ -219,6 +227,52 @@ def expand_(it: GKLIterator, state: GKLFactorization) -> GKLFactorization:
     state.k += 1
     state.r = r
     return state
+
+
+def expand_many_(it: GKLIterator, state: GKLFactorization, nsteps: int, tol: float, check=None) -> int:
+    """Up to `nsteps` consecutive expand! steps, stopping after the first one with normres <= tol or a non-finite
+    coefficient; returns the number of steps done.  With `it.pair` and ClassicalGramSchmidt2 or the flagged
+    ModifiedGramSchmidt2Blocked they are chained on the device in one C-ABI call (b2k_gkl_expand_many, one host
+    synchronisation); every other iterator steps through gklrecurrence, calling `check(state)` after each step.
+    The chained steps are committed before an error is raised, like lanczos.expand_many_."""
+    if nsteps <= 0:
+        return 0
+    U, V, r = state.U, state.V, state.r
+    k = len(U)
+    chained = it.pair is not None and it.orth.tag in (L.CGS2, L.MGS2B)
+    if not chained or k + nsteps > CHAIN_COLS[r.ctx.np_dtype.itemsize]:
+        done = 0
+        for _ in range(nsteps):
+            expand_(it, state)
+            done += 1
+            if check is not None:
+                check(state)
+            a, b = state.alphas[-1], state.betas[-1]
+            if b <= tol or not (math.isfinite(a) and math.isfinite(b)):
+                break
+        return done
+    A, At = it.pair
+    ctx = r.ctx
+    ucols = (L.c_vec * (k + nsteps + 1))(*[u.handle for u in U.basis], r.handle)
+    vcols = (L.c_vec * (k + nsteps))(*[v.handle for v in V.basis])
+    al = (C.c_double * nsteps)()
+    be = (C.c_double * nsteps)()
+    done, rout = C.c_int32(), L.c_vec()
+    status = ctx.lib.b2k_gkl_expand_many(ctx.h, A.h, At.h, ucols, vcols, k, nsteps, state.normres(), tol,
+                                         it.orth.tag, al, be, C.byref(done), C.byref(rout))
+    d = done.value
+    if d > 0:
+        r.disown()                                  # released (and possibly reused) inside the library
+        for i in range(d):
+            U.push(B200Vec(ctx, ucols[k + i]))      # columns allocated by the library
+            V.push(B200Vec(ctx, vcols[k + i]))
+        state.r = B200Vec(ctx, rout.value)
+        state.alphas.extend(al[:d])
+        state.betas.extend(be[:d])
+        state.k += d
+        state.passes += 2 * d
+    ctx.check(status)
+    return d
 
 
 def shrink_(state: GKLFactorization, k: int) -> GKLFactorization:
