@@ -148,12 +148,26 @@ int32_t b2k_vec_axpy2(b2k_ctx* ctx, b2k_vec y, b2k_vec x1, double a1, b2k_vec x2
 /* apply(A::AbstractMatrix, x) = A*x — src/apply.jl:1.  CSR, 0-based, int32 indices on
  * device.  rowptr/colidx given as int64 or int32 host arrays (idx_bytes = 8 or 4),
  * `index_base` 0 or 1.  vals are of the context dtype.  In a dist context the rows are
- * the local rows and colidx are GLOBAL columns; the halo plan is built here. */
+ * the local rows and colidx are GLOBAL columns; the halo plan is built here.  The stored
+ * order is kept (unsorted and repeated columns included).  Refused, with *out left
+ * untouched: idx_bytes not 4 / 8 or index_base not 0 / 1 (B2K_EINVAL); a negative n_rows,
+ * n_cols or nnz (B2K_EINVAL); local n_rows or nnz >= 2^31, or on a single GPU n_cols
+ * >= 2^31 (B2K_ENOTSUP; a dist context's n_cols is the global column count, which may
+ * be larger); n_rows that is not the length of space 0 (dist) or of any space
+ * (B2K_EDIM); rowptr[0] != base,
+ * rowptr[n_rows] != nnz + base, an entry outside [base, nnz + base] or a decreasing
+ * rowptr (B2K_EINVAL); a column outside [base, n_cols + base) (B2K_EINVAL; n_global in
+ * a dist context). */
 int32_t b2k_op_create_csr(b2k_ctx* ctx, b2k_op** out, int64_t n_rows, int64_t n_cols,
                           int64_t nnz, const void* rowptr, const void* colidx,
                           const void* vals, int32_t idx_bytes, int32_t index_base);
 /* Julia SparseMatrixCSC (colptr, rowval, nzval; 1-based Int64) — converted to CSR of A
- * (transposed on the host once).  Single-GPU contexts only. */
+ * (transposed on the host once: within a row, columns ascending, a repeated entry in
+ * colptr order).  rowval / nzval may be longer than nnz; the entries past nnz are never
+ * read.  Single-GPU contexts only (B2K_ENOTSUP).  Refused, with *out left untouched:
+ * idx_bytes / index_base as for CSR; the sizes and rows as for CSR; colptr[0] != base,
+ * colptr[n_cols] != nnz + base or a decreasing colptr (B2K_EINVAL); a row outside
+ * [base, n_rows + base) (B2K_EINVAL). */
 int32_t b2k_op_create_csc(b2k_ctx* ctx, b2k_op** out, int64_t n_rows, int64_t n_cols,
                           int64_t nnz, const void* colptr, const void* rowval,
                           const void* nzval, int32_t idx_bytes, int32_t index_base);

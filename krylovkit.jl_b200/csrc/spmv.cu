@@ -1338,10 +1338,13 @@ int32_t build_compact(b2k_ctx* ctx, b2k_op* op) {
     return B2K_OK;
 }
 
-int32_t finish_csr(b2k_ctx* ctx, b2k_op* op) {
+// rowptr_bad: k_convert_rowptr's out-of-range flag when nothing has read it back yet (an operator without nonzeros
+// has no column check); it comes back with the stats, so such an operator pays no synchronisation of its own.
+int32_t finish_csr(b2k_ctx* ctx, b2k_op* op, const unsigned long long* rowptr_bad = nullptr) {
     const int64_t n = op->n_rows;
     int* d_stats;
     int h_stats[2] = {0, 0};
+    unsigned long long h_bad = 0;
     B2K_CUDA(ctx, B2K_DMALLOC(&d_stats, 2 * sizeof(int)));
     B2K_CUDA(ctx, cudaMemsetAsync(d_stats, 0, 2 * sizeof(int), ctx->stream));
     if (n > 0) {
@@ -1349,8 +1352,11 @@ int32_t finish_csr(b2k_ctx* ctx, b2k_op* op) {
         B2K_LAUNCH_CHECK(ctx);
     }
     B2K_CUDA(ctx, cudaMemcpyAsync(h_stats, d_stats, sizeof(h_stats), cudaMemcpyDeviceToHost, ctx->stream));
+    if (rowptr_bad)
+        B2K_CUDA(ctx, cudaMemcpyAsync(&h_bad, rowptr_bad, sizeof(h_bad), cudaMemcpyDeviceToHost, ctx->stream));
     B2K_TRY(b2k_stream_sync(ctx));
     B2K_DFREE(d_stats);
+    if (h_bad != 0) return b2k_fail(ctx, B2K_EINVAL, "op_create_csr: rowptr entry outside [base, nnz + base]");
     if (h_stats[1] != 0) return b2k_fail(ctx, B2K_EINVAL, "CSR: rowptr is not non-decreasing");
     const int maxrow = h_stats[0];
     if (maxrow <= SP_NNZ / 2) {
@@ -1382,13 +1388,18 @@ int32_t finish_csr(b2k_ctx* ctx, b2k_op* op) {
     return B2K_OK;
 }
 
-// raw host index arrays (int32/int64, base 0/1) -> device rowptr (int32) / global columns (int64)
+// raw host index arrays (int32/int64, base 0/1) -> device rowptr (int32) / global columns (int64).  A row pointer
+// outside [base, nnz + base] sets *bad: the test runs on the raw value, as the int32 cast can make an int64 entry
+// look in range and monotone.
 template <typename IT>
 __global__ void k_convert_rowptr(const IT* __restrict__ raw, int base, int32_t* __restrict__ out,
-                                 int64_t count) {
+                                 int64_t count, int64_t nnz, unsigned long long* __restrict__ bad) {
     for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < count;
-         i += (int64_t)gridDim.x * blockDim.x)
-        out[i] = (int32_t)((int64_t)raw[i] - base);
+         i += (int64_t)gridDim.x * blockDim.x) {
+        const int64_t v = (int64_t)raw[i];
+        if (v < base || v > nnz + base) *bad = 1ull;
+        out[i] = (int32_t)(v - base);
+    }
 }
 template <typename IT>
 __global__ void k_convert_cols(const IT* __restrict__ raw, int base, int64_t* __restrict__ out,
@@ -1494,19 +1505,33 @@ void widen(const void* src, int64_t count, int base, std::vector<int64_t>* out) 
 
 // Upload raw index arrays and do all conversion / validation / planning on the device:
 // host work is O(1), so a host-buffer eigsolve pays only the PCIe copies.
-static int32_t create_csr_raw(b2k_ctx* ctx, b2k_op** out, int64_t n_rows, int64_t n_cols,
-                              int64_t nnz, const void* rowptr, const void* colidx,
-                              const void* vals, int32_t idx_bytes, int32_t index_base) {
-    if (nnz >= (int64_t)1 << 31 || n_rows >= (int64_t)1 << 31)
-        return b2k_fail(ctx, B2K_ENOTSUP, "CSR: nnz/rows per GPU must be < 2^31");
-    // rows must be the length of a vector space of this context: space 0 in general, any space for a
-    // rectangular operator on a single GPU (the (A, A') pair of lssolve / svdsolve)
+// Shapes of an operator built from index arrays: no negative size; rows and nnz per GPU below 2^31 (the device
+// indices are int32), and so the columns on one GPU, where k_localize_cols stores the column itself (a row shard's
+// columns are global, and become local or halo indices that fit); the rows the length of a vector space of this
+// context: space 0 in general, any space for a rectangular operator on a single GPU (the (A, A') pair of lssolve /
+// svdsolve).
+static int32_t check_index_shape(b2k_ctx* ctx, const char* who, int64_t n_rows, int64_t n_cols, int64_t nnz) {
+    if (n_rows < 0 || n_cols < 0 || nnz < 0)
+        return b2k_fail(ctx, B2K_EINVAL, "%s: negative size (%lld rows, %lld columns, nnz %lld)", who,
+                        (long long)n_rows, (long long)n_cols, (long long)nnz);
+    const int64_t lim = (int64_t)1 << 31;
+    if (n_rows >= lim || nnz >= lim)
+        return b2k_fail(ctx, B2K_ENOTSUP, "%s: rows and nnz per GPU must be < 2^31", who);
+    if (ctx->nranks == 1 && n_cols >= lim)
+        return b2k_fail(ctx, B2K_ENOTSUP, "%s: columns on one GPU must be < 2^31", who);
     bool rows_ok = n_rows == ctx->spaces[0].n;
     if (!rows_ok && ctx->nranks == 1)
         for (const auto& sp : ctx->spaces) rows_ok = rows_ok || sp.n == n_rows;
     if (!rows_ok)
-        return b2k_fail(ctx, B2K_EDIM, "CSR: %lld local rows but space 0 holds %lld",
+        return b2k_fail(ctx, B2K_EDIM, "%s: %lld local rows but space 0 holds %lld", who,
                         (long long)n_rows, (long long)ctx->spaces[0].n);
+    return B2K_OK;
+}
+
+static int32_t create_csr_raw(b2k_ctx* ctx, b2k_op** out, int64_t n_rows, int64_t n_cols,
+                              int64_t nnz, const void* rowptr, const void* colidx,
+                              const void* vals, int32_t idx_bytes, int32_t index_base) {
+    B2K_TRY(check_index_shape(ctx, "op_create_csr", n_rows, n_cols, nnz));
     const int64_t rp0 = idx_bytes == 8 ? ((const int64_t*)rowptr)[0] : ((const int32_t*)rowptr)[0];
     const int64_t rpn = idx_bytes == 8 ? ((const int64_t*)rowptr)[n_rows] : ((const int32_t*)rowptr)[n_rows];
     if (rp0 - index_base != 0 || rpn - index_base != nnz)
@@ -1519,6 +1544,7 @@ static int32_t create_csr_raw(b2k_ctx* ctx, b2k_op** out, int64_t n_rows, int64_
     op->nnz = nnz;
     int64_t* d_gcol = nullptr;
     void* d_raw = nullptr;
+    unsigned long long* d_chk = nullptr;      // {min column, max column, a row pointer out of range}
     const int64_t nnz1 = std::max<int64_t>(1, nnz);
     const size_t raw_bytes = (size_t)idx_bytes * std::max<int64_t>(nnz1, n_rows + 1);
     int32_t rc = B2K_OK;
@@ -1526,6 +1552,7 @@ static int32_t create_csr_raw(b2k_ctx* ctx, b2k_op** out, int64_t n_rows, int64_
         cudaStreamSynchronize(ctx->stream);
         if (d_gcol) B2K_DFREE(d_gcol);
         if (d_raw) B2K_DFREE(d_raw);
+        if (d_chk) B2K_DFREE(d_chk);
         b2k_op_destroy(ctx, op);
         return code;
     };
@@ -1541,10 +1568,13 @@ static int32_t create_csr_raw(b2k_ctx* ctx, b2k_op** out, int64_t n_rows, int64_
     CK(B2K_DMALLOC(&op->vals, (size_t)ctx->esize * (nnz1 + 8)));
     CK(B2K_DMALLOC(&d_gcol, sizeof(int64_t) * nnz1));
     CK(B2K_DMALLOC(&d_raw, raw_bytes));
+    CK(B2K_DMALLOC(&d_chk, 3 * sizeof(unsigned long long)));
+    unsigned long long chk[3] = {~0ull, 0ull, 0ull};
+    CK(cudaMemcpyAsync(d_chk, chk, sizeof(chk), cudaMemcpyHostToDevice, ctx->stream));
     const int g = ctx->num_sms * 8;
     CK(cudaMemcpyAsync(d_raw, rowptr, (size_t)idx_bytes * (n_rows + 1), cudaMemcpyHostToDevice, ctx->stream));
-    if (idx_bytes == 8) k_convert_rowptr<int64_t><<<g, 256, 0, ctx->stream>>>((const int64_t*)d_raw, index_base, op->rowptr, n_rows + 1);
-    else k_convert_rowptr<int32_t><<<g, 256, 0, ctx->stream>>>((const int32_t*)d_raw, index_base, op->rowptr, n_rows + 1);
+    if (idx_bytes == 8) k_convert_rowptr<int64_t><<<g, 256, 0, ctx->stream>>>((const int64_t*)d_raw, index_base, op->rowptr, n_rows + 1, nnz, d_chk + 2);
+    else k_convert_rowptr<int32_t><<<g, 256, 0, ctx->stream>>>((const int32_t*)d_raw, index_base, op->rowptr, n_rows + 1, nnz, d_chk + 2);
     ctx->launches++;
     if (nnz > 0) {
         CK(cudaMemcpyAsync(d_raw, colidx, (size_t)idx_bytes * nnz, cudaMemcpyHostToDevice, ctx->stream));
@@ -1553,29 +1583,31 @@ static int32_t create_csr_raw(b2k_ctx* ctx, b2k_op** out, int64_t n_rows, int64_
         ctx->launches++;
         CK(cudaMemcpyAsync(op->vals, vals, (size_t)ctx->esize * nnz, cudaMemcpyHostToDevice, ctx->stream));
         // validate the column range on the device
-        unsigned long long* d_mm;
-        CK(B2K_DMALLOC(&d_mm, 2 * sizeof(unsigned long long)));
-        unsigned long long init[2] = {~0ull, 0ull}, mm[2];
-        CK(cudaMemcpyAsync(d_mm, init, sizeof(init), cudaMemcpyHostToDevice, ctx->stream));
-        k_minmax_cols<<<ctx->num_sms * 4, 256, 0, ctx->stream>>>(d_gcol, nnz, d_mm, d_mm + 1);
+        k_minmax_cols<<<ctx->num_sms * 4, 256, 0, ctx->stream>>>(d_gcol, nnz, d_chk, d_chk + 1);
         ctx->launches++;
-        CK(cudaMemcpyAsync(mm, d_mm, sizeof(mm), cudaMemcpyDeviceToHost, ctx->stream));
+        // one read-back for both checks; nothing that indexes with these arrays has run yet
+        CK(cudaMemcpyAsync(chk, d_chk, sizeof(chk), cudaMemcpyDeviceToHost, ctx->stream));
         CK(cudaStreamSynchronize(ctx->stream));
-        B2K_DFREE(d_mm);
+        if (chk[2] != 0)
+            return fail(b2k_fail(ctx, B2K_EINVAL, "op_create_csr: rowptr entry outside [%d, nnz + %d]", index_base,
+                                 index_base));
         const int64_t colmax = ctx->nranks > 1 ? ctx->n_global : n_cols;
         // negative columns wrap to huge unsigned values and are caught by the max test
-        if ((int64_t)mm[1] >= colmax || (int64_t)mm[1] < 0)
+        if ((int64_t)chk[1] >= colmax || (int64_t)chk[1] < 0)
             return fail(b2k_fail(ctx, B2K_EINVAL, "op_create_csr: column index out of range [0, %lld)",
                                  (long long)colmax));
     }
 #undef CK
+    // without nonzeros, plan_halo and localize read no index array, and finish_csr reads the flag back before it
+    // uses rowptr for anything but its stats (which read in bounds whatever the values)
     rc = plan_halo(ctx, op, d_gcol);
     if (rc == B2K_OK) rc = localize(ctx, op, d_gcol);
-    if (rc == B2K_OK) rc = finish_csr(ctx, op);
+    if (rc == B2K_OK) rc = finish_csr(ctx, op, nnz > 0 ? nullptr : d_chk + 2);
     if (rc != B2K_OK) return fail(rc);
     cudaStreamSynchronize(ctx->stream);
     B2K_DFREE(d_gcol);
     B2K_DFREE(d_raw);
+    B2K_DFREE(d_chk);
     ctx->ops.push_back(op);
     *out = op;
     return B2K_OK;
@@ -1597,14 +1629,18 @@ extern "C" int32_t b2k_op_create_csc(b2k_ctx* ctx, b2k_op** out, int64_t n_rows,
     if (ctx->nranks > 1) return b2k_fail(ctx, B2K_ENOTSUP, "op_create_csc: single-GPU contexts only");
     if ((idx_bytes != 4 && idx_bytes != 8) || (index_base != 0 && index_base != 1))
         return b2k_fail(ctx, B2K_EINVAL, "op_create_csc: idx_bytes must be 4/8, index_base 0/1");
+    B2K_TRY(check_index_shape(ctx, "op_create_csc", n_rows, n_cols, nnz));
     std::vector<int64_t> cp, rv;
-    if (idx_bytes == 8) {
-        widen<int64_t>(colptr, n_cols + 1, index_base, &cp);
-        widen<int64_t>(rowval, nnz, index_base, &rv);
-    } else {
-        widen<int32_t>(colptr, n_cols + 1, index_base, &cp);
-        widen<int32_t>(rowval, nnz, index_base, &rv);
-    }
+    if (idx_bytes == 8) widen<int64_t>(colptr, n_cols + 1, index_base, &cp);
+    else widen<int32_t>(colptr, n_cols + 1, index_base, &cp);
+    // the loops below index rowval / nzval and the rows' fill positions through colptr: check it first
+    bool cp_ok = cp[0] == 0 && cp[n_cols] == nnz;
+    for (int64_t c = 0; c < n_cols && cp_ok; ++c) cp_ok = cp[c] <= cp[c + 1];
+    if (!cp_ok)
+        return b2k_fail(ctx, B2K_EINVAL, "op_create_csc: colptr must rise from %d to nnz + %d", index_base,
+                        index_base);
+    if (idx_bytes == 8) widen<int64_t>(rowval, nnz, index_base, &rv);
+    else widen<int32_t>(rowval, nnz, index_base, &rv);
     // counting-sort transpose: CSC(A) -> CSR(A); within a row, columns come out ascending
     std::vector<int64_t> rp(n_rows + 1, 0), gc(nnz);
     for (int64_t i = 0; i < nnz; ++i) {

@@ -69,8 +69,9 @@ class B200CSR(B200Operator):
 
     @classmethod
     def from_scipy(cls, ctx: B200Context, A) -> "B200CSR":
-        A = A.tocsr()
-        A.sort_indices()
+        A = A.tocsr()                      # the caller's own matrix when it is CSR already: never sorted in place
+        if not A.has_sorted_indices:
+            A = A.sorted_indices()
         n_rows, n_cols = A.shape
         rp = np.ascontiguousarray(A.indptr, dtype=np.int64)
         ci = np.ascontiguousarray(A.indices, dtype=np.int64)
@@ -96,12 +97,18 @@ class B200CSR(B200Operator):
 
     @classmethod
     def from_julia_csc(cls, ctx: B200Context, m, n, colptr, rowval, nzval) -> "B200CSR":
-        """SparseMatrixCSC fields as Julia stores them (1-based Int64)."""
+        """SparseMatrixCSC fields as Julia stores them (1-based Int64).  nnz is colptr[n] - 1, as Julia's `nnz`:
+        rowval and nzval may carry spare capacity past it."""
         cp = np.ascontiguousarray(colptr, dtype=np.int64)
         rv = np.ascontiguousarray(rowval, dtype=np.int64)
         nz = np.ascontiguousarray(nzval, dtype=ctx.np_dtype)
+        if n < 0 or len(cp) != n + 1:
+            raise L.B200Error(f"from_julia_csc: colptr has {len(cp)} entries, {n} columns need {n + 1}")
+        nnz = int(cp[-1]) - 1
+        if len(rv) < nnz or len(nz) < nnz:
+            raise L.B200Error(f"from_julia_csc: colptr holds {nnz} entries, rowval {len(rv)} and nzval {len(nz)}")
         h = L.c_op()
-        ctx.check(ctx.lib.b2k_op_create_csc(ctx.h, C.byref(h), m, n, len(nz), cp.ctypes.data,
+        ctx.check(ctx.lib.b2k_op_create_csc(ctx.h, C.byref(h), m, n, nnz, cp.ctypes.data,
                                             rv.ctypes.data, nz.ctypes.data, 8, 1))
         return cls(ctx, h)
 

@@ -336,28 +336,66 @@ class HostSimLib:
         _set(out, self.next_id)
         return L.OK
 
+    def _index_shape(self, ctx, who, idx_bytes, index_base, n_rows, n_cols, nnz):
+        """the library's refusals of an index-array operator, in its order, before any array is read"""
+        if idx_bytes not in (4, 8) or index_base not in (0, 1):
+            return self._fail(ctx, L.EINVAL, f"{who}: idx_bytes must be 4/8, index_base 0/1")
+        if min(n_rows, n_cols, nnz) < 0:
+            return self._fail(ctx, L.EINVAL, f"{who}: negative size")
+        if max(n_rows, nnz) >= 1 << 31:
+            return self._fail(ctx, L.ENOTSUP, f"{who}: rows and nnz per GPU must be < 2^31")
+        if ctx.dist is None and n_cols >= 1 << 31:        # a row shard's n_cols is the global column count
+            return self._fail(ctx, L.ENOTSUP, f"{who}: columns on one GPU must be < 2^31")
+        if n_rows != ctx.spaces[0].n and (ctx.dist is not None or not any(s.n == n_rows for s in ctx.spaces)):
+            return self._fail(ctx, L.EDIM, f"{who}: {n_rows} local rows but space 0 holds {ctx.spaces[0].n}")
+        return L.OK
+
+    @staticmethod
+    def _ptr_ok(p, count):
+        """p (int64, base removed) runs from 0 to count, never decreasing"""
+        return p[0] == 0 and p[-1] == count and bool(np.all(np.diff(p) >= 0))
+
     def b2k_op_create_csr(self, h, out, n_rows, n_cols, nnz, rowptr, colidx, vals, idx_bytes, index_base):
         ctx = self._c(h)
+        st = self._index_shape(ctx, "op_create_csr", idx_bytes, index_base, n_rows, n_cols, nnz)
+        if st != L.OK:
+            return st
         it = C.c_int64 if idx_bytes == 8 else C.c_int32
-        rp = np.array(_view(rowptr, n_rows + 1, it)) - index_base
-        ci = np.array(_view(colidx, nnz, it)) - index_base
-        va = np.array(_view(vals, nnz, ctx.ctype))
-        if not any(s.n == n_rows for s in ctx.spaces):
-            return self._fail(ctx, L.EDIM, f"CSR: {n_rows} local rows but space 0 holds {ctx.spaces[0].n}")
+        rp = np.array(_view(rowptr, n_rows + 1, it), dtype=np.int64) - index_base
+        if not self._ptr_ok(rp, nnz):
+            return self._fail(ctx, L.EINVAL, "op_create_csr: rowptr does not rise from 0 to nnz")
+        ci = np.array(_view(colidx, nnz, it), dtype=np.int64) - index_base
         if ctx.dist is not None:                      # local rows, GLOBAL column indices
             n_cols = ctx.dist["n_global"]
+        if nnz > 0 and (ci.min() < 0 or ci.max() >= n_cols):
+            return self._fail(ctx, L.EINVAL, f"op_create_csr: column index out of range [0, {n_cols})")
+        va = np.array(_view(vals, nnz, ctx.ctype))
         return self._newop(out, sp.csr_matrix((va, ci, rp), shape=(n_rows, n_cols)))
 
     def b2k_op_create_csc(self, h, out, n_rows, n_cols, nnz, colptr, rowval, nzval, idx_bytes, index_base):
         ctx = self._c(h)
+        if ctx.dist is not None:
+            return self._fail(ctx, L.ENOTSUP, "op_create_csc: single-GPU contexts only")
+        st = self._index_shape(ctx, "op_create_csc", idx_bytes, index_base, n_rows, n_cols, nnz)
+        if st != L.OK:
+            return st
         it = C.c_int64 if idx_bytes == 8 else C.c_int32
-        cp = np.array(_view(colptr, n_cols + 1, it)) - index_base
-        rv = np.array(_view(rowval, nnz, it)) - index_base
+        cp = np.array(_view(colptr, n_cols + 1, it), dtype=np.int64) - index_base
+        if not self._ptr_ok(cp, nnz):
+            return self._fail(ctx, L.EINVAL, "op_create_csc: colptr does not rise from 0 to nnz")
+        rv = np.array(_view(rowval, nnz, it), dtype=np.int64) - index_base
+        if nnz > 0 and (rv.min() < 0 or rv.max() >= n_rows):
+            return self._fail(ctx, L.EINVAL, "op_create_csc: row index out of range")
         nz = np.array(_view(nzval, nnz, ctx.ctype))
         return self._newop(out, sp.csc_matrix((nz, rv, cp), shape=(n_rows, n_cols)).tocsr())
 
     def b2k_op_create_stencil(self, h, out, nx, ny, nz, c):
         ctx = self._c(h)
+        if min(nx, ny, nz) < 1:
+            return self._fail(ctx, L.EINVAL, "stencil: bad grid")
+        nglob = ctx.dist["n_global"] if ctx.dist is not None else ctx.spaces[0].n
+        if nx * ny * nz != nglob:
+            return self._fail(ctx, L.EDIM, f"stencil: grid has {nx * ny * nz} points, the operator needs {nglob}")
         A = ko.stencil_matrix(nx, ny, nz, tuple(float(c[i]) for i in range(7)), dtype=ctx.dtype)
         if ctx.dist is not None:                      # this rank's rows of the global operator
             r0 = ctx.dist["row_offset"]
@@ -366,6 +404,10 @@ class HostSimLib:
 
     def b2k_op_create_dense(self, h, out, m, n, host, ld):
         ctx = self._c(h)
+        if ld < m or m < 1 or n < 1:
+            return self._fail(ctx, L.EINVAL, "dense: bad shape")
+        if m != ctx.spaces[0].n:
+            return self._fail(ctx, L.EDIM, f"dense: {m} local rows but space 0 holds {ctx.spaces[0].n}")
         A = np.array(_view(host, ld * n, ctx.ctype)).reshape(n, ld).T[:m, :]
         return self._newop(out, np.array(A))
 
