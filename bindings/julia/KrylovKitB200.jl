@@ -539,6 +539,29 @@ function minres_chain!(A::B200CSR, x::B200Vec, p_prev::B200Vec, p_cur::B200Vec, 
     copyto!(state, out)
     return rec[:, 1:done[]]
 end
+# lsmr_chain!: up to `nsteps` LSMR iterations (lsmr.jl:61-149) for min ‖b − A x‖² + λ²‖x‖² with one host
+# synchronisation.  At (b2k_op_create_transpose) is A's exact transpose; `ring` holds max(krylovdim, 1) columns of the
+# spare column's space in slot order, v_{iter0+1} normalised in slot iter0 % length(ring), u normalised; av is work
+# space.  `state` is (α, β, ᾱ, ρ, ρ̄, c̄, s̄, θ, ζ̄, λ) — (α, β, α, 1, 1, 1, 0, 0, αβ, λ) at the start — and is advanced in
+# place.  Returns a 16 × done matrix, one column per iteration: (α, β, ρ, ρ̄, θ, ζ, |ζ̄|, stop code, Aᵀ applied, ᾱ, c̄, s̄,
+# g, ζ/(ρρ̄), 0, 0); stop code 1: |ζ̄| ≤ tol, 2: β ≤ tol (v stays in its slot, u unnormalised), 3: α ≤ tol (v is the
+# unnormalised spare column), 4: a non-finite scalar.  Otherwise v is in slot (iter0 + done) % length(ring).
+function lsmr_chain!(A::B200CSR, At::B200CSR, x::B200Vec, h::B200Vec, hbar::B200Vec, r::B200Vec, Ah::B200Vec,
+                     Ahbar::B200Vec, u::B200Vec, av::B200Vec, ring::Vector{<:B200Vec}, krylovdim::Integer,
+                     spare::B200Vec, orth::Integer, iter0::Integer, state::Vector{Float64}, tol::Real,
+                     nsteps::Integer)
+    rec, done, out = zeros(Float64, 16, nsteps), Ref{Int32}(0), zeros(Float64, 10)
+    hs = Int32[v.handle for v in ring]
+    check(x.ctx.h, ccall((:b2k_lsmr_chain, lib), Cint,
+                         (Ptr{Cvoid}, Ptr{Cvoid}, Ptr{Cvoid}, Int32, Int32, Int32, Int32, Int32, Int32, Int32, Int32,
+                          Ptr{Int32}, Int32, Int32, Int32, Int32, Ptr{Float64}, Float64, Int32, Ptr{Float64},
+                          Ptr{Float64}, Ref{Int32}),
+                         x.ctx.h, A.h, At.h, x.handle, h.handle, hbar.handle, r.handle, Ah.handle, Ahbar.handle,
+                         u.handle, av.handle, hs, Int32(krylovdim), spare.handle, Int32(orth), Int32(iter0), state,
+                         Float64(tol), Int32(nsteps), rec, out, done))
+    copyto!(state, out)
+    return rec[:, 1:done[]]
+end
 # KrylovKit.linsolve(A::B200CSR, b, x₀, alg::MINRES, a₀, a₁): KrylovKit declares `MINRES` and has no method for it; the
 # driver is krylovkit.jl_b200/linsolve.py::_minres, statement for statement — initial residual, batches of
 # minres_chain!, the explicit residual behind every |φ̄| < tol, restart from x when it disagrees.

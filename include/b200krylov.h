@@ -314,6 +314,43 @@ int32_t b2k_minres_chain(b2k_ctx* ctx, const b2k_op* op, b2k_vec x, b2k_vec p_pr
                          b2k_vec d1, b2k_vec d2, double a0, double a1, const double* state_in, double tol,
                          int32_t nsteps, double* rec_out, double* state_out, int32_t* steps_done);
 
+/* Up to `nsteps` (1 <= nsteps <= B2K_MAX_CHAIN - 1) LSMR iterations (src/lssolve/lsmr.jl:61-149, with lambda) for
+ * min ||b - A x||^2 + lambda^2 ||x||^2, A a stored CSR matrix (m x n) and At its exact transpose
+ * (b2k_op_create_transpose), enqueued back to back with ONE host synchronisation per call.  Per iteration: the A
+ * SpMV (gathering v = v~/alpha), one streaming pass over the m-vectors (Ah-bar, r, Ah, u~, beta), the A' SpMV
+ * (gathering u = u~/beta; skipped when beta <= tol), one streaming pass over the n-vectors (v into its ring slot,
+ * h-bar, x, h, v~ = A'u - beta v); with krylovdim > 1 the reorthogonalisation of v~ against the ring in slot order
+ * (ModifiedGramSchmidt / ModifiedGramSchmidt2: the pipelined MGS sweep once / twice; ClassicalGramSchmidt2 /
+ * ModifiedGramSchmidt2Blocked: two passes of the cooperative classical sweep) and a norm pass.  The scalar recurrence runs on the device
+ * in Float64; the updates it drives are applied one iteration late, and two flush launches apply the last ones.
+ * Vectors: x, h, hbar, spare (length n); r, Ah, Ahbar, u, av (length m; av is work space); ring: max(krylovdim, 1)
+ * columns of the spare column's space, in slot order.  ON ENTRY AND ON RETURN the vectors are those of the
+ * reference loop at the top of iteration iter0 + 1: u normalised, v_{iter0+1} normalised in ring slot
+ * iter0 % max(krylovdim, 1), no update pending.  After a call that ran d = *steps_done iterations, iter0 + d is the
+ * next call's iter0.  The last iteration's stop code moves v (the reference's `v`): code 2 (beta <= tol) keeps
+ * v_k in its slot and leaves u unnormalised; code 3 (alpha <= tol) leaves v unnormalised in the SPARE column and
+ * the ring untouched; otherwise v is in slot (iter0 + d) % max(krylovdim, 1).
+ * state_in / state_out, 10 doubles: {alpha, beta, alphabar, rho, rhobar, cbar, sbar, theta, zetabar, lambda}; the
+ * reference's loop starts from {alpha, beta, alpha, 1, 1, 1, 0, 0, alpha*beta, lambda}.  Handing state_out to the
+ * next call continues the same process bit for bit.
+ * rec_out: 16 doubles per completed iteration {alpha, beta, rho, rhobar, theta, zeta, |zetabar|, stop code,
+ * A' applied (0 / 1), alphabar, cbar, sbar, g, zeta/(rho rhobar), 0, 0}; stop code 1 = |zetabar| <= tol, 2 = beta <=
+ * tol, 3 = alpha <= tol, 4 = a non-finite scalar.  A beta / alpha breakdown is completed as the reference completes
+ * it, and the chain stops after it; the stopping iteration is the last of *steps_done.
+ * Rounding: every vector is rounded exactly like the scale!! / add!! it replaces, given the same scalars; beta and
+ * (krylovdim <= 1) alpha are CTA-ordered sums, which may differ from b2k_vec_norm in the last bits, and the three
+ * rotations spell hypot out as sqrt(a*a + b*b) with every operation rounded on its own (it overflows once an
+ * argument exceeds about 1.3e154).  The chained and the step-by-step loop therefore agree to rounding, not bit for
+ * bit.  A refused call writes nothing: B2K_ENOTSUP for a row-sharded context, an operator that is not a stored CSR
+ * matrix, krylovdim > 1 with another orthogonalizer, krylovdim > 128 or (CGS2 / MGS2B) more ring columns than the
+ * sweep's panel ring holds; B2K_EDIM when At is not A's shape transposed, a vector has the wrong length, or the m-vectors (r, Ah, Ahbar,
+ * u, av) or the n-vectors (x, h, hbar, spare, ring) are not columns of one space each;
+ * B2K_EINVAL for null pointers, two handles of one vector, nsteps outside 1 .. B2K_MAX_CHAIN - 1 or iter0 < 0. */
+int32_t b2k_lsmr_chain(b2k_ctx* ctx, const b2k_op* A, const b2k_op* At, b2k_vec x, b2k_vec h, b2k_vec hbar,
+                       b2k_vec r, b2k_vec Ah, b2k_vec Ahbar, b2k_vec u, b2k_vec av, const b2k_vec* ring,
+                       int32_t krylovdim, b2k_vec spare, int32_t alg, int32_t iter0, const double* state_in,
+                       double tol, int32_t nsteps, double* rec_out, double* state_out, int32_t* steps_done);
+
 /* ---------------------------------------------- basis (OrthonormalBasis) ---- */
 /* project!!(y, b, x, alpha, beta, r): h[j] = beta*h[j] + alpha*<b[cols[j]], x>
  * — src/orthonormal.jl:88-118.  h is a HOST vector (orthonormal.jl:374, arnoldi.jl:212). */

@@ -113,6 +113,9 @@ _PROTOS = {
                            [C.c_int32, P(C.c_double), P(C.c_int32)]),
     "b2k_minres_chain": (C.c_int32, [c_ctx, c_op] + [c_vec] * 6 + [C.c_double, C.c_double, P(C.c_double), C.c_double,
                                      C.c_int32, P(C.c_double), P(C.c_double), P(C.c_int32)]),
+    "b2k_lsmr_chain": (C.c_int32, [c_ctx, c_op, c_op] + [c_vec] * 8 + [P(c_vec), C.c_int32, c_vec, C.c_int32, C.c_int32,
+                                  P(C.c_double), C.c_double, C.c_int32, P(C.c_double), P(C.c_double),
+                                  P(C.c_int32)]),
     "b2k_basis_project": (C.c_int32, [c_ctx, P(c_vec), C.c_int32, c_vec, C.c_double, C.c_double,
                                       P(C.c_double)]),
     "b2k_basis_cross_inner": (C.c_int32, [c_ctx, P(c_vec), C.c_int32, P(c_vec), C.c_int32, C.c_int32, C.c_int32,

@@ -1880,9 +1880,11 @@ bool chain_ok(const b2k_ctx* ctx, const b2k_op* op, const b2k_vec* cols, int32_t
 // The cooperative CGS sweep of one chained step over the K1 columns of pn, finalised into the device record rec.
 // Lanczos: with the three-term prologue (beta from rec_prev, <v, A v> from rec).  GKL (b2k_gkl_expand_many): no
 // prologue (the SpMV epilogue has subtracted alpha u already), and a non-finite norm raises the stop flag too.
+// skip_on (b2k_lsmr_chain): the device flag that makes the launch do nothing, instead of the batch's stop flag.
 template <typename T>
 int32_t chain_step_gs(b2k_ctx* ctx, const Panel& pn, int K1, const VecRef& rw, double* rec_prev, double* rec,
-                      double tol, const PeerStep* psp, bool prologue = true, int stop_nonfinite = 0) {
+                      double tol, const PeerStep* psp, bool prologue = true, int stop_nonfinite = 0,
+                      const int* skip_on = nullptr) {
     const int grid = grid_for_rows<T>(ctx, pn.n);
     ColList cl;
     lanczos_cols(cl, pn, K1, prologue);
@@ -1893,7 +1895,7 @@ int32_t chain_step_gs(b2k_ctx* ctx, const Panel& pn, int K1, const VecRef& rw, d
     lanczos_sweeps<T>(ctx, fp, pn, K1, rw, grid, prologue, 0.0, 0.0, prologue ? rec_prev + 2 : nullptr,
                       prologue ? rec + 0 : nullptr);
     fp.fin.stop_nonfinite = stop_nonfinite;
-    fp.stop = reinterpret_cast<const int*>(ctx->d_sync + B2K_SYNC_STOP);
+    fp.stop = skip_on ? skip_on : reinterpret_cast<const int*>(ctx->d_sync + B2K_SYNC_STOP);
     fp.trace = ctx->d_trace;
     fp.fin.A = PA; fp.fin.B = nullptr; fp.fin.N = PN; fp.fin.G = grid; fp.fin.stride = B2K_KSTRIDE;
     fp.fin.k = K1; fp.fin.res = nullptr; fp.fin.off = 0; fp.fin.noff = 0; fp.fin.rec = rec;
@@ -2286,6 +2288,171 @@ extern "C" int32_t b2k_gkl_expand_many(b2k_ctx* ctx, const b2k_op* A, const b2k_
     B2K_TRY(gkl_refuse(ctx, A, At, ucols, vcols, k, nsteps, alg));
     return gkl_chain(ctx, A, At, ucols, vcols, k, nsteps, beta_old, tol, alg, alphas_out, betas_out, steps_done,
                      r_out);
+}
+
+// ---------------------------------------------------------------------------------------
+// Device-chained LSMR iterations (lsmr.jl:61-149), b2k_lsmr_chain.  Per iteration k, with one host synchronisation
+// per call:
+//   1. A SpMV (m rows): gathers v_k = rn(src * (1/alpha_k)) (xscale) into the work column Av;
+//   2. k_lsmr_m: iteration k-1's Ah-bar / r tail, Ah, u~_{k+1} = Av - alpha_k u_k, beta_{k+1} (last CTA);
+//   3. A' SpMV (n rows): gathers u_{k+1} = rn(u~ * (1/beta)); does nothing when beta <= tol (skip flag);
+//   4. k_lsmr_n: v_k into its ring slot, iteration k-1's h-bar / x / h tail, v~_{k+1} = y - beta v_k in the spare
+//      column; without reorthogonalisation it also sums v~^2 and runs the scalar recurrence in its last CTA;
+//   5. (krylovdim > 1) the reorthogonalisation of v~_{k+1} against the ring in slot order — the pipelined MGS sweep
+//      once or twice, or two passes of the cooperative classical sweep — then k_lsmr_alpha: alpha and the recurrence.
+// Two flush launches (one per side) apply the tail of the last iteration that ran and normalise u and v.
+namespace {
+
+int32_t lsmr_refuse(b2k_ctx* ctx, const b2k_op* A, const b2k_op* At, const VecRef* mv, const VecRef* nv,
+                    const VecRef* rr, int nring, int32_t krylovdim, int32_t alg) {
+    if (ctx->nranks > 1) return b2k_fail(ctx, B2K_ENOTSUP, "lsmr_chain: row-sharded contexts are not supported");
+    int64_t m = 0, n = 0, tm = 0, tn = 0;
+    int32_t ka = -1, kt = -1;
+    B2K_TRY(b2k_op_info(A, &m, &n, nullptr, &ka));
+    B2K_TRY(b2k_op_info(At, &tm, &tn, nullptr, &kt));
+    if (ka != 0 || kt != 0) return b2k_fail(ctx, B2K_ENOTSUP, "lsmr_chain: A and A' must be stored CSR matrices");
+    const bool gs = alg == B2K_CGS2 || alg == B2K_MGS2B;
+    if (krylovdim > 1) {
+        if (alg != B2K_MGS && alg != B2K_MGS2 && !gs)
+            return b2k_fail(ctx, B2K_ENOTSUP, "lsmr_chain: orthogonalizer %d does not chain with krylovdim > 1", alg);
+        const int C = ctx->dtype == B2K_F64 ? 8 : 16;
+        if (gs && (!g_use_coop || (nring + C - 1) / C > NS || nring > MAXCH * C))
+            return b2k_fail(ctx, B2K_ENOTSUP, "lsmr_chain: %d ring columns do not fit the sweep's panel ring", nring);
+    }
+    if (nring > LS_MAXRING)
+        return b2k_fail(ctx, B2K_ENOTSUP, "lsmr_chain: krylovdim %d > %d", krylovdim, LS_MAXRING);
+    if (tm != n || tn != m)
+        return b2k_fail(ctx, B2K_EDIM, "lsmr_chain: A' is %lld x %lld, A is %lld x %lld", (long long)tm, (long long)tn,
+                        (long long)m, (long long)n);
+    for (int i = 0; i < 5; ++i)
+        if (mv[i].n != m) return b2k_fail(ctx, B2K_EDIM, "lsmr_chain: r, Ah, Ah-bar, u, Av must have length %lld",
+                                          (long long)m);
+    for (int i = 0; i < 4; ++i)
+        if (nv[i].n != n) return b2k_fail(ctx, B2K_EDIM, "lsmr_chain: x, h, h-bar, spare must have length %lld",
+                                          (long long)n);
+    for (int i = 1; i < 5; ++i)
+        if (mv[i].space != mv[0].space)
+            return b2k_fail(ctx, B2K_EDIM, "lsmr_chain: r, Ah, Ah-bar, u, Av must be columns of one space");
+    for (int i = 0; i < 3; ++i)
+        if (nv[i].space != nv[3].space)
+            return b2k_fail(ctx, B2K_EDIM, "lsmr_chain: x, h, h-bar and the spare must be columns of one space");
+    for (int i = 0; i < nring; ++i)
+        if (rr[i].n != n || rr[i].space != nv[3].space)
+            return b2k_fail(ctx, B2K_EDIM, "lsmr_chain: the ring and the spare column must be columns of one space of "
+                                           "length %lld", (long long)n);
+    // every vector is written by some launch while others read: no two handles may share storage
+    std::vector<const VecRef*> all;
+    for (int i = 0; i < 5; ++i) all.push_back(mv + i);
+    for (int i = 0; i < 4; ++i) all.push_back(nv + i);
+    for (int i = 0; i < nring; ++i) all.push_back(rr + i);
+    for (size_t i = 0; i < all.size(); ++i)
+        for (size_t j = 0; j < i; ++j)
+            if (all[i]->ptr == all[j]->ptr)
+                return b2k_fail(ctx, B2K_EINVAL, "lsmr_chain: vectors %zu and %zu are the same", j, i);
+    return B2K_OK;
+}
+
+}  // namespace
+
+extern "C" int32_t b2k_lsmr_chain(b2k_ctx* ctx, const b2k_op* A, const b2k_op* At, b2k_vec x, b2k_vec h,
+                                  b2k_vec hbar, b2k_vec r, b2k_vec Ah, b2k_vec Ahbar, b2k_vec u, b2k_vec av,
+                                  const b2k_vec* ring, int32_t krylovdim, b2k_vec spare, int32_t alg, int32_t iter0,
+                                  const double* state_in, double tol, int32_t nsteps, double* rec_out,
+                                  double* state_out, int32_t* steps_done) {
+    if (!ctx) return B2K_EINVAL;
+    if (!A || !At || !ring || !state_in || !rec_out || !state_out || !steps_done)
+        return b2k_fail(ctx, B2K_EINVAL, "lsmr_chain: null pointer");
+    if (nsteps < 1 || nsteps > B2K_MAX_CHAIN - 1 || iter0 < 0)
+        return b2k_fail(ctx, B2K_EINVAL, "lsmr_chain: need 1 <= nsteps <= %d and iter0 >= 0", B2K_MAX_CHAIN - 1);
+    const int nring = krylovdim > 1 ? krylovdim : 1;
+    if (nring > LS_MAXRING) return b2k_fail(ctx, B2K_ENOTSUP, "lsmr_chain: krylovdim %d > %d", krylovdim, LS_MAXRING);
+    VecRef mv[5], nv[4];
+    std::vector<VecRef> rr(nring);
+    const b2k_vec mh[5] = {r, Ah, Ahbar, u, av}, nh[4] = {x, h, hbar, spare};
+    for (int i = 0; i < 5; ++i) B2K_TRY(b2k_resolve(ctx, mh[i], &mv[i]));
+    for (int i = 0; i < 4; ++i) B2K_TRY(b2k_resolve(ctx, nh[i], &nv[i]));
+    for (int i = 0; i < nring; ++i) B2K_TRY(b2k_resolve(ctx, ring[i], &rr[i]));
+    B2K_TRY(lsmr_refuse(ctx, A, At, mv, nv, rr.data(), nring, krylovdim, alg));
+    *steps_done = 0;
+    const int64_t m = mv[0].n, n = nv[0].n;
+    const bool f64 = ctx->dtype == B2K_F64;
+    LsmrDev d;
+    memset(&d, 0, sizeof(d));
+    d.st = ctx->d_steps;
+    d.rec0 = ctx->d_steps + LS_NSTATE;
+    d.stop = reinterpret_cast<int*>(ctx->d_sync + B2K_SYNC_STOP);
+    d.skip = reinterpret_cast<int*>(ctx->d_sync + B2K_SYNC_SKIP);
+    d.tol = tol;
+    d.iter0 = iter0;
+    d.nring = nring;
+    for (int i = 0; i < nring; ++i) d.ring[i] = rr[i].ptr;
+    double seed[LS_NSTATE] = {};
+    memcpy(seed, state_in, LS_NIO * sizeof(double));
+    seed[LS_INVA] = 1.0;                           // u and v are normalised on entry
+    seed[LS_INVB] = 1.0;
+    B2K_TRY(b2k_put_coef(ctx, seed, LS_NSTATE, 0));
+    B2K_CUDA(ctx, cudaMemcpyAsync(d.st, ctx->d_coef, LS_NSTATE * sizeof(double), cudaMemcpyDeviceToDevice, ctx->stream));
+    B2K_CUDA(ctx, cudaMemsetAsync(d.rec0, 0, sizeof(double) * LS_REC * nsteps, ctx->stream));
+    B2K_CUDA(ctx, cudaMemsetAsync(d.stop, 0, sizeof(int), ctx->stream));
+    B2K_CUDA(ctx, cudaMemsetAsync(d.skip, 0, sizeof(int), ctx->stream));
+    SpmvFuse fa, ft;
+    memset(&fa, 0, sizeof(fa));
+    fa.stop = d.stop;
+    fa.xscale = d.st + LS_INVA;
+    ft = fa;
+    ft.stop = d.skip;
+    ft.xscale = d.st + LS_INVB;
+    const bool reorth = krylovdim > 1;
+    int32_t rc = B2K_OK;
+    for (int32_t i = 0; i < nsteps && rc == B2K_OK; ++i) {
+        const int k = iter0 + 1 + i;               // v_k sits (or will sit) in ring slot (k - 1) % nring
+        const VecRef& P = rr[(k - 1) % nring];
+        const VecRef& src = i == 0 ? P : nv[3];
+        const VecRef& yv = i == 0 ? nv[3] : P;
+        if ((rc = b2k_enqueue_apply_fused(ctx, A, src, mv[4], 0.0, 1.0, false, nullptr, nullptr, &fa)) != B2K_OK) break;
+        if ((rc = b2k_lsmr_enqueue_m(ctx, m, mv[0].ptr, mv[1].ptr, mv[2].ptr, mv[3].ptr, mv[4].ptr, i > 0, false, d)) != B2K_OK)
+            break;
+        if ((rc = b2k_enqueue_apply_fused(ctx, At, mv[3], yv, 0.0, 1.0, false, nullptr, nullptr, &ft)) != B2K_OK) break;
+        if ((rc = b2k_lsmr_enqueue_n(ctx, n, nv[0].ptr, nv[1].ptr, nv[2].ptr, P.ptr, nv[3].ptr, i > 0, i > 0, !reorth, d)) !=
+            B2K_OK)
+            break;
+        if (!reorth) continue;
+        const int cnt = std::min(krylovdim, k);    // V holds v_1 .. v_k, at most krylovdim of them, in slot order
+        Panel pn;
+        if ((rc = make_panel(ctx, ring, cnt, &pn)) != B2K_OK) break;
+        if (alg == B2K_MGS || alg == B2K_MGS2) {
+            ctx->dot_stop = d.skip;
+            rc = mgs_sweep(ctx, pn, nv[3], cnt, 0, -1);
+            if (rc == B2K_OK && alg == B2K_MGS2) rc = mgs_sweep(ctx, pn, nv[3], cnt, cnt, -1);
+            ctx->dot_stop = nullptr;
+        } else {                                   // orthogonalize!! with CGS2: two classical passes
+            for (int ps = 0; ps < 2 && rc == B2K_OK; ++ps)
+                rc = f64 ? chain_step_gs<double>(ctx, pn, cnt, nv[3], nullptr, d.st + LS_FIN, -INFINITY, nullptr, false, 0,
+                                                 d.skip)
+                         : chain_step_gs<float>(ctx, pn, cnt, nv[3], nullptr, d.st + LS_FIN, -INFINITY, nullptr, false, 0,
+                                                d.skip);
+        }
+        if (rc == B2K_OK) rc = b2k_lsmr_enqueue_alpha(ctx, n, nv[3].ptr, d);
+    }
+    if (rc != B2K_OK) {                            // nothing is reported from a call that could not be enqueued
+        cudaStreamSynchronize(ctx->stream);
+        return rc;
+    }
+    B2K_TRY(b2k_lsmr_enqueue_m(ctx, m, mv[0].ptr, mv[1].ptr, mv[2].ptr, mv[3].ptr, nullptr, true, true, d));
+    B2K_TRY(b2k_lsmr_enqueue_flush_n(ctx, n, nv[0].ptr, nv[1].ptr, nv[2].ptr, nv[3].ptr, d));
+    B2K_CUDA(ctx, cudaMemcpyAsync(ctx->h_res, d.rec0, sizeof(double) * LS_REC * nsteps, cudaMemcpyDeviceToHost,
+                                  ctx->stream));
+    double* hst = ctx->h_res + B2K_RES_DOUBLES - LS_NSTATE / 2;
+    static_assert(LS_NIO <= LS_NSTATE / 2, "state block");
+    B2K_CUDA(ctx, cudaMemcpyAsync(hst, d.st, sizeof(double) * LS_NIO, cudaMemcpyDeviceToHost, ctx->stream));
+    B2K_TRY(b2k_stream_sync(ctx));
+    int32_t dn = nsteps;
+    for (int32_t i = 0; i < nsteps; ++i)
+        if (ctx->h_res[(size_t)LS_REC * i + 7] != 0.0) { dn = i + 1; break; }
+    memcpy(rec_out, ctx->h_res, sizeof(double) * LS_REC * dn);
+    memcpy(state_out, hst, sizeof(double) * LS_NIO);
+    *steps_done = dn;
+    return B2K_OK;
 }
 
 extern "C" int32_t b2k_basis_transform(b2k_ctx* ctx, const b2k_vec* cols, int32_t m,

@@ -232,13 +232,17 @@ __global__ void __launch_bounds__(BT) k_givens(T* __restrict__ q1, T* __restrict
 // with s_prev read from d_res[src] (device scalar of the previous reduction).  That is the
 // pipelined MGS step (orthonormal.jl:417-421): v -= s_{j-1} q_{j-1}; s_j = <q_j, v>.
 // FINAL: 0 = raw sum, 1 = sqrt(sum)
-template <typename T, bool UPDATE, bool NORM>
+// STOP (the MGS sweeps of b2k_lsmr_chain): the launch does nothing once *stop is raised.
+template <typename T, bool UPDATE, bool NORM, bool STOP = false>
 __global__ void __launch_bounds__(BT)
 k_dot(const T* __restrict__ q, T* __restrict__ x, int64_t n, const T* __restrict__ qprev,
       const double* __restrict__ sprev, double* __restrict__ part, unsigned* __restrict__ ticket,
-      double* __restrict__ out, double* __restrict__ accum_into, int hints) {
+      double* __restrict__ out, double* __restrict__ accum_into, int hints, const int* stop) {
     __shared__ double red[32];
     __shared__ bool last;
+    if constexpr (STOP) {
+        if (*reinterpret_cast<const volatile int*>(stop)) return;
+    }
     // hints (the MGS sweep): x is re-read and re-written once per basis column — keep it in L2 (evict_last);
     // the basis columns pass once (evict_first)
     const uint64_t pol_keep = hints ? l2_policy_evict_last() : 0, pol_once = hints ? l2_policy_evict_first() : 0;
@@ -295,9 +299,12 @@ k_dot(const T* __restrict__ q, T* __restrict__ x, int64_t n, const T* __restrict
 }
 
 // final fix-up: x <- x - s*q with s = d_res[src] (tail of the pipelined MGS sweep)
-template <typename T>
+template <typename T, bool STOP = false>
 __global__ void __launch_bounds__(BT)
-k_axpy_dev(T* __restrict__ x, const T* __restrict__ q, const double* __restrict__ s, int64_t n) {
+k_axpy_dev(T* __restrict__ x, const T* __restrict__ q, const double* __restrict__ s, int64_t n, const int* stop) {
+    if constexpr (STOP) {
+        if (*reinterpret_cast<const volatile int*>(stop)) return;
+    }
     const T sp = (T)(*s);
     constexpr int V = Vec16<T>::N;
     const int64_t nv = n / V;
@@ -689,7 +696,363 @@ k_minres_step(T* __restrict__ x, T* pA, T* pB, const T* __restrict__ q, T* dA, T
     });
 }
 
+// ---- LSMR (lsmr.jl:61-149; b2k_lsmr_chain) ----
+// add!!(y, x, 1, b) as k_axpby rounds it: b == 0 gives x (MODE 0), otherwise fma(1, x, rn(b y)) (MODE 1 and 2).
+template <typename T>
+__device__ __forceinline__ T axpy1_rn(T x, T b, bool bzero, T y) {
+    return bzero ? x : fma((T)1, x, mul_rn(b, y));
+}
+
+// sqrt(a^2 + b^2) with every product and sum rounded on its own (the host restatement's plain double arithmetic);
+// overflows once a or b exceeds about 1.3e154, where hypot would not
+__device__ __forceinline__ double hyp_rn(double a, double b) {
+    return __dsqrt_rn(__dadd_rn(__dmul_rn(a, a), __dmul_rn(b, b)));
+}
+
+// The scalar half of one LSMR iteration (lsmr.jl:92-113 with lambda), one thread, Float64, in the operation order of
+// lssolve.py::_lsmr (so a host restatement in plain double arithmetic gives the same bits).  nrm2 = ||v~||^2 of this
+// iteration (ignored when beta <= tol: alpha and v are kept).  Writes the record of the iteration and the state the
+// pending updates and the next iteration read; raises the stop flags on a stop code.
+__device__ void lsmr_recurrence(const LsmrDev& d, double nrm2) {
+    volatile double* w = d.st;
+    const bool bskip = w[LS_BSKIP] != 0.0;
+    const double beta = w[LS_BETA];
+    const double alpha = bskip ? w[LS_ALPHA] : __dsqrt_rn(nrm2);
+    const double lam = w[LS_LAM], rhoold = w[LS_RHO], rhobarold = w[LS_RHOBAR];
+    const double cbar0 = w[LS_CBAR], sbar0 = w[LS_SBAR], zetabar0 = w[LS_ZETABAR];
+    const double alphahat = hyp_rn(w[LS_ALPHABAR], lam);
+    const double rho = hyp_rn(alphahat, beta);
+    const double c = __ddiv_rn(alphahat, rho), s = __ddiv_rn(beta, rho);
+    const double theta = __dmul_rn(s, alpha);
+    const double alphabar = __dmul_rn(c, alpha);
+    const double thetabar = __dmul_rn(sbar0, rho);
+    const double cbarrho = __dmul_rn(cbar0, rho);
+    const double rhobar = hyp_rn(cbarrho, theta);
+    const double cbar = __ddiv_rn(cbarrho, rhobar), sbar = __ddiv_rn(theta, rhobar);
+    const double zeta = __dmul_rn(cbar, zetabar0);
+    const double zetabar = __dmul_rn(-sbar, zetabar0);
+    const double g = __ddiv_rn(__dmul_rn(-thetabar, rho), __dmul_rn(rhoold, rhobarold));
+    const double cz = __ddiv_rn(zeta, __dmul_rn(rho, rhobar));
+    const bool askip = !bskip && !(alpha > d.tol);
+    const bool finite = isfinite(alpha) && isfinite(beta) && isfinite(rho) && isfinite(rhobar) && isfinite(g) &&
+                        isfinite(cz) && isfinite(zetabar);
+    const double code = fabs(zetabar) <= d.tol ? 1.0 : bskip ? 2.0 : askip ? 3.0 : !finite ? 4.0 : 0.0;
+    const int done = (int)w[LS_DONE];
+    double* rec = d.rec0 + (size_t)LS_REC * done;
+    rec[0] = alpha; rec[1] = beta; rec[2] = rho; rec[3] = rhobar; rec[4] = theta; rec[5] = zeta; rec[6] = fabs(zetabar);
+    rec[7] = code; rec[8] = bskip ? 0.0 : 1.0; rec[9] = alphabar; rec[10] = cbar; rec[11] = sbar; rec[12] = g;
+    rec[13] = cz;
+    w[LS_ALPHA] = alpha; w[LS_ALPHABAR] = alphabar; w[LS_RHO] = rho; w[LS_RHOBAR] = rhobar; w[LS_CBAR] = cbar;
+    w[LS_SBAR] = sbar; w[LS_THETA] = theta; w[LS_ZETABAR] = zetabar;
+    w[LS_INVA] = (bskip || askip) ? 1.0 : __ddiv_rn(1.0, alpha);
+    w[LS_G] = g; w[LS_CZ] = cz; w[LS_ASKIP] = askip ? 1.0 : 0.0;
+    w[LS_DONE] = (double)(done + 1);
+    if (code != 0.0) {
+        *d.stop = 1;
+        *d.skip = 1;
+    }
+}
+
+// The u side of iteration k (m rows), after Av = A v_k:
+//   pend:  Ah-bar <- add!!(Ah-bar, Ah, 1, g);  r <- add!!(r, Ah-bar, -zeta/(rho rhobar))   [iteration k-1's tail]
+//          Ah <- add!!(Ah, Av, 1, -theta/rho);  u~ <- add!!(Av, rn(u~ (1/beta)), -alpha), sum u~^2
+// u~ stays unnormalised; the last CTA writes beta_{k+1}, 1/beta_{k+1} and the A'-side skip flag (beta <= tol).
+// FLUSH: only the pending tail, and u <- rn(u~ (1/beta)) unless beta <= tol (the reference leaves u unscaled then).
+template <typename T, bool FLUSH>
+__global__ void __launch_bounds__(BT)
+k_lsmr_m(T* __restrict__ r, T* __restrict__ Ah, T* __restrict__ Ahb, T* __restrict__ u, const T* __restrict__ Av,
+         int64_t n, bool pend, double* __restrict__ part, unsigned* __restrict__ ticket, const LsmrDev d) {
+    __shared__ double red[32];
+    __shared__ bool last;
+    if (!FLUSH && *reinterpret_cast<const volatile int*>(d.stop)) return;
+    const volatile double* st = d.st;
+    const double gd = st[LS_G], tr = __ddiv_rn(-st[LS_THETA], st[LS_RHO]);
+    const T g = (T)gd, ncz = (T)(-st[LS_CZ]), ntr = (T)tr, na = (T)(-st[LS_ALPHA]), ib = (T)st[LS_INVB];
+    const bool gz = gd == 0.0, tz = tr == 0.0;
+    const bool su = !FLUSH || st[LS_BSKIP] == 0.0;
+    constexpr int V = Vec16<T>::N;
+    const int64_t nv = n / V;
+    const int64_t stride = (int64_t)gridDim.x * BT;
+    T acc = 0;
+    auto each = [&](T& rv, T& ahv, T& hbv, T& uv, T avv) {
+        if (pend) {
+            hbv = axpy1_rn(ahv, g, gz, hbv);
+            rv = fma(ncz, hbv, rv);
+        }
+        if (!FLUSH) {
+            ahv = axpy1_rn(avv, ntr, tz, ahv);
+            uv = fma(na, mul_rn(uv, ib), avv);
+            acc = fma(uv, uv, acc);
+        } else if (su) {
+            uv = mul_rn(uv, ib);
+        }
+    };
+    B2K_TRIP(2) {
+        T rv[2][V] = {}, ahv[2][V], hbv[2][V] = {}, uv[2][V], avv[2][V] = {};
+        B2K_EACH(2, q, i) {
+            vload<T>(Ah + i * V, ahv[q]);
+            vload<T>(u + i * V, uv[q]);
+            if (pend) {
+                vload<T>(r + i * V, rv[q]);
+                vload<T>(Ahb + i * V, hbv[q]);
+            }
+            if (!FLUSH) vload<T>(Av + i * V, avv[q]);
+        }
+        B2K_EACH(2, q, i) {
+#pragma unroll
+            for (int j = 0; j < V; ++j) each(rv[q][j], ahv[q][j], hbv[q][j], uv[q][j], avv[q][j]);
+            if (pend) {
+                vstore<T>(r + i * V, rv[q]);
+                vstore<T>(Ahb + i * V, hbv[q]);
+            }
+            if (!FLUSH) vstore<T>(Ah + i * V, ahv[q]);
+            if (su) vstore<T>(u + i * V, uv[q]);
+        }
+    }
+    if (blockIdx.x == 0 && threadIdx.x < (n - nv * V)) {
+        const int64_t i = nv * V + threadIdx.x;
+        T rv = pend ? r[i] : (T)0, ahv = Ah[i], hbv = pend ? Ahb[i] : (T)0, uv = u[i];
+        each(rv, ahv, hbv, uv, FLUSH ? (T)0 : Av[i]);
+        if (pend) {
+            r[i] = rv;
+            Ahb[i] = hbv;
+        }
+        if (!FLUSH) Ah[i] = ahv;
+        if (su) u[i] = uv;
+    }
+    if (FLUSH) return;
+    finish_sums<1>({block_sum((double)acc, red)}, part, ticket, red, &last, BT, [&](int, double tot) {
+        const double beta = __dsqrt_rn(tot);
+        const bool bskip = !(beta > d.tol);
+        double* w = d.st;
+        w[LS_BETA] = beta;
+        w[LS_INVB] = __ddiv_rn(1.0, beta);
+        w[LS_BSKIP] = bskip ? 1.0 : 0.0;
+        *d.skip = bskip ? 1 : 0;
+    });
+}
+
+// The v side of iteration k (n rows), after y = A' u_{k+1} (skipped when beta <= tol).  P is v_k's ring slot; the
+// operand source and y are (P, Q) in the first iteration of a call (v_k normalised in its slot, y in the spare column
+// Q) and (Q, P) after it (v~_k unnormalised in Q, y in the slot v_k replaces):
+//   v_k = rn(src (1/alpha_k)) -> P
+//   pend: h-bar <- add!!(h-bar, h, 1, g); x <- add!!(x, h-bar, zeta/(rho rhobar)); h <- add!!(h, v_k, 1, -theta/rho)
+//   unless beta <= tol: v~_{k+1} = add!!(y, v_k, -beta) -> Q
+// NORM (no reorthogonalisation): sum v~_{k+1}^2, and the last CTA runs the recurrence.
+template <typename T, bool NORM>
+__global__ void __launch_bounds__(BT)
+k_lsmr_n(T* __restrict__ x, T* __restrict__ h, T* __restrict__ hb, T* P, T* Q, int64_t n, bool swap, bool pend,
+         double* __restrict__ part, unsigned* __restrict__ ticket, const LsmrDev d) {
+    __shared__ double red[32];
+    __shared__ bool last;
+    if (*reinterpret_cast<const volatile int*>(d.stop)) return;
+    const volatile double* st = d.st;
+    const double gd = st[LS_G], tr = __ddiv_rn(-st[LS_THETA], st[LS_RHO]);
+    const T g = (T)gd, cz = (T)st[LS_CZ], ntr = (T)tr, ia = (T)st[LS_INVA], nb = (T)(-st[LS_BETA]);
+    const bool gz = gd == 0.0, tz = tr == 0.0, bskip = st[LS_BSKIP] != 0.0;
+    const T* src = swap ? Q : P;
+    const T* yv = swap ? P : Q;
+    constexpr int V = Vec16<T>::N;
+    const int64_t nv = n / V;
+    const int64_t stride = (int64_t)gridDim.x * BT;
+    T acc = 0;
+    auto each = [&](T sv, T y, T& xv, T& hv, T& hbv, T& vout, T& tout) {
+        const T v = mul_rn(sv, ia);
+        vout = v;
+        if (pend) {
+            hbv = axpy1_rn(hv, g, gz, hbv);
+            xv = fma(cz, hbv, xv);
+            hv = axpy1_rn(v, ntr, tz, hv);
+        }
+        if (!bskip) {
+            tout = fma(nb, v, y);
+            if (NORM) acc = fma(tout, tout, acc);
+        }
+    };
+    B2K_TRIP(2) {
+        T sv[2][V], y[2][V] = {}, xv[2][V] = {}, hv[2][V] = {}, hbv[2][V] = {}, vo[2][V], to[2][V] = {};
+        B2K_EACH(2, q, i) {
+            vload<T>(src + i * V, sv[q]);
+            if (!bskip) vload<T>(yv + i * V, y[q]);
+            if (pend) {
+                vload<T>(x + i * V, xv[q]);
+                vload<T>(h + i * V, hv[q]);
+                vload<T>(hb + i * V, hbv[q]);
+            }
+        }
+        B2K_EACH(2, q, i) {
+#pragma unroll
+            for (int j = 0; j < V; ++j) each(sv[q][j], y[q][j], xv[q][j], hv[q][j], hbv[q][j], vo[q][j], to[q][j]);
+            if (swap) vstore<T>(P + i * V, vo[q]);
+            if (!bskip) vstore<T>(Q + i * V, to[q]);
+            if (pend) {
+                vstore<T>(x + i * V, xv[q]);
+                vstore<T>(h + i * V, hv[q]);
+                vstore<T>(hb + i * V, hbv[q]);
+            }
+        }
+    }
+    if (blockIdx.x == 0 && threadIdx.x < (n - nv * V)) {
+        const int64_t i = nv * V + threadIdx.x;
+        T xv = pend ? x[i] : (T)0, hv = pend ? h[i] : (T)0, hbv = pend ? hb[i] : (T)0, vo, to = 0;
+        each(src[i], bskip ? (T)0 : yv[i], xv, hv, hbv, vo, to);
+        if (swap) P[i] = vo;
+        if (!bskip) Q[i] = to;
+        if (pend) {
+            x[i] = xv;
+            h[i] = hv;
+            hb[i] = hbv;
+        }
+    }
+    if (!NORM) return;
+    finish_sums<1>({block_sum((double)acc, red)}, part, ticket, red, &last, BT,
+                   [&](int, double tot) { lsmr_recurrence(d, tot); });
+}
+
+// alpha after the reorthogonalisation (K > 1): the CTA-ordered sum of v~^2, then the recurrence in the last CTA
+template <typename T>
+__global__ void __launch_bounds__(BT)
+k_lsmr_alpha(const T* __restrict__ Q, int64_t n, double* __restrict__ part, unsigned* __restrict__ ticket,
+             const LsmrDev d) {
+    __shared__ double red[32];
+    __shared__ bool last;
+    if (*reinterpret_cast<const volatile int*>(d.stop)) return;
+    if (d.st[LS_BSKIP] != 0.0) {             // alpha and v are kept: no sum
+        if (blockIdx.x == 0 && threadIdx.x == 0) lsmr_recurrence(d, 0.0);
+        return;
+    }
+    constexpr int V = Vec16<T>::N;
+    const int64_t nv = n / V;
+    const int64_t stride = (int64_t)gridDim.x * BT;
+    T acc = 0;
+    B2K_TRIP(4) {
+        T a[4][V];
+        B2K_EACH(4, q, i) vload<T>(Q + i * V, a[q]);
+        B2K_EACH(4, q, i) {
+#pragma unroll
+            for (int j = 0; j < V; ++j) acc = fma(a[q][j], a[q][j], acc);
+        }
+    }
+    if (blockIdx.x == 0 && threadIdx.x < (n - nv * V)) {
+        const T t = Q[nv * V + threadIdx.x];
+        acc = fma(t, t, acc);
+    }
+    finish_sums<1>({block_sum((double)acc, red)}, part, ticket, red, &last, BT,
+                   [&](int, double tot) { lsmr_recurrence(d, tot); });
+}
+
+// The flush of the v side: the tail of the last iteration k that ran, whether or not the chain has stopped.
+// v_{k+1} = rn(v~ (1/alpha)) into ring slot k % nring; beta <= tol: v is v_k, already in slot (k-1) % nring;
+// alpha <= tol: v is v~ itself, left in the spare column.  Then the pending h-bar, x, h updates with that v.
+template <typename T>
+__global__ void __launch_bounds__(BT)
+k_lsmr_flush_n(T* __restrict__ x, T* __restrict__ h, T* __restrict__ hb, T* spare, int64_t n,
+               const __grid_constant__ LsmrDev d) {
+    const volatile double* st = d.st;
+    const int k = d.iter0 + (int)st[LS_DONE];
+    const bool bskip = st[LS_BSKIP] != 0.0, askip = st[LS_ASKIP] != 0.0;
+    const T* src = bskip ? (const T*)d.ring[(k - 1) % d.nring] : spare;
+    T* dst = (bskip || askip) ? nullptr : (T*)d.ring[k % d.nring];
+    const double gd = st[LS_G], tr = __ddiv_rn(-st[LS_THETA], st[LS_RHO]);
+    const T g = (T)gd, cz = (T)st[LS_CZ], ntr = (T)tr, ia = (T)st[LS_INVA];
+    const bool gz = gd == 0.0, tz = tr == 0.0;
+    constexpr int V = Vec16<T>::N;
+    const int64_t nv = n / V;
+    const int64_t stride = (int64_t)gridDim.x * BT;
+    auto each = [&](T sv, T& xv, T& hv, T& hbv, T& vout) {
+        const T v = mul_rn(sv, ia);
+        vout = v;
+        hbv = axpy1_rn(hv, g, gz, hbv);
+        xv = fma(cz, hbv, xv);
+        hv = axpy1_rn(v, ntr, tz, hv);
+    };
+    B2K_TRIP(2) {
+        T sv[2][V], xv[2][V], hv[2][V], hbv[2][V], vo[2][V];
+        B2K_EACH(2, q, i) {
+            vload<T>(src + i * V, sv[q]);
+            vload<T>(x + i * V, xv[q]);
+            vload<T>(h + i * V, hv[q]);
+            vload<T>(hb + i * V, hbv[q]);
+        }
+        B2K_EACH(2, q, i) {
+#pragma unroll
+            for (int j = 0; j < V; ++j) each(sv[q][j], xv[q][j], hv[q][j], hbv[q][j], vo[q][j]);
+            if (dst) vstore<T>(dst + i * V, vo[q]);
+            vstore<T>(x + i * V, xv[q]);
+            vstore<T>(h + i * V, hv[q]);
+            vstore<T>(hb + i * V, hbv[q]);
+        }
+    }
+    if (blockIdx.x == 0 && threadIdx.x < (n - nv * V)) {
+        const int64_t i = nv * V + threadIdx.x;
+        T xv = x[i], hv = h[i], hbv = hb[i], vo;
+        each(src[i], xv, hv, hbv, vo);
+        if (dst) dst[i] = vo;
+        x[i] = xv;
+        h[i] = hv;
+        hb[i] = hbv;
+    }
+}
+
 }  // namespace
+
+// ---- LSMR chain launches (b2k_lsmr_chain, basis.cu) ----
+int32_t b2k_lsmr_enqueue_m(b2k_ctx* ctx, int64_t m, void* r, void* Ah, void* Ahbar, void* u, const void* Av,
+                           bool pend, bool flush, const LsmrDev& d) {
+    const int grid = grid_for(ctx, m, 4);
+#define LAUNCH(T, FL)                                                                                               \
+    k_lsmr_m<T, FL><<<grid, BT, 0, ctx->stream>>>((T*)r, (T*)Ah, (T*)Ahbar, (T*)u, (const T*)Av, m, pend,         \
+                                                  ctx->d_part_s, ctx->d_sync, d)
+    if (ctx->dtype == B2K_F64) {
+        if (flush) LAUNCH(double, true);
+        else LAUNCH(double, false);
+    } else {
+        if (flush) LAUNCH(float, true);
+        else LAUNCH(float, false);
+    }
+#undef LAUNCH
+    B2K_LAUNCH_CHECK(ctx);
+    return B2K_OK;
+}
+
+int32_t b2k_lsmr_enqueue_n(b2k_ctx* ctx, int64_t n, void* x, void* h, void* hbar, void* P, void* Q, bool swap,
+                           bool pend, bool norm, const LsmrDev& d) {
+    const int grid = grid_for(ctx, n, 4);
+#define LAUNCH(T, NR)                                                                                               \
+    k_lsmr_n<T, NR><<<grid, BT, 0, ctx->stream>>>((T*)x, (T*)h, (T*)hbar, (T*)P, (T*)Q, n, swap, pend,            \
+                                                  ctx->d_part_s, ctx->d_sync, d)
+    if (ctx->dtype == B2K_F64) {
+        if (norm) LAUNCH(double, true);
+        else LAUNCH(double, false);
+    } else {
+        if (norm) LAUNCH(float, true);
+        else LAUNCH(float, false);
+    }
+#undef LAUNCH
+    B2K_LAUNCH_CHECK(ctx);
+    return B2K_OK;
+}
+
+int32_t b2k_lsmr_enqueue_alpha(b2k_ctx* ctx, int64_t n, const void* Q, const LsmrDev& d) {
+    const int grid = grid_for(ctx, n, 8);
+    if (ctx->dtype == B2K_F64)
+        k_lsmr_alpha<double><<<grid, BT, 0, ctx->stream>>>((const double*)Q, n, ctx->d_part_s, ctx->d_sync, d);
+    else
+        k_lsmr_alpha<float><<<grid, BT, 0, ctx->stream>>>((const float*)Q, n, ctx->d_part_s, ctx->d_sync, d);
+    B2K_LAUNCH_CHECK(ctx);
+    return B2K_OK;
+}
+
+int32_t b2k_lsmr_enqueue_flush_n(b2k_ctx* ctx, int64_t n, void* x, void* h, void* hbar, void* spare,
+                                 const LsmrDev& d) {
+    const int grid = grid_for(ctx, n, 4);
+    if (ctx->dtype == B2K_F64)
+        k_lsmr_flush_n<double><<<grid, BT, 0, ctx->stream>>>((double*)x, (double*)h, (double*)hbar, (double*)spare, n, d);
+    else
+        k_lsmr_flush_n<float><<<grid, BT, 0, ctx->stream>>>((float*)x, (float*)h, (float*)hbar, (float*)spare, n, d);
+    B2K_LAUNCH_CHECK(ctx);
+    return B2K_OK;
+}
 
 // ------------------------------------------------------------------ internal API ----
 // Enqueue: d_res[slot] = <q, x> (or ||x||^2 if q == nullptr), optionally after the fused
@@ -702,9 +1065,15 @@ int32_t b2k_enqueue_dot(b2k_ctx* ctx, const void* q, void* x, int64_t n, const v
     double* acc = accum_slot >= 0 ? ctx->d_res + accum_slot : nullptr;
     const double* sp = sprev_slot >= 0 ? ctx->d_res + sprev_slot : nullptr;
     unsigned* ticket = ctx->d_sync;
-#define LAUNCH(T, UPD, NRM)                                                              \
-    k_dot<T, UPD, NRM><<<grid, BT, 0, ctx->stream>>>((const T*)q, (T*)x, n, (const T*)qprev, \
-                                                     sp, ctx->d_part_s, ticket, out, acc, ctx->dot_hints)
+#define LAUNCH_S(T, UPD, NRM, ST)                                                                    \
+    k_dot<T, UPD, NRM, ST><<<grid, BT, 0, ctx->stream>>>((const T*)q, (T*)x, n, (const T*)qprev, sp,         \
+                                                         ctx->d_part_s, ticket, out, acc, ctx->dot_hints,   \
+                                                         ctx->dot_stop)
+#define LAUNCH(T, UPD, NRM)                          \
+    do {                                             \
+        if (ctx->dot_stop) LAUNCH_S(T, UPD, NRM, true); \
+        else LAUNCH_S(T, UPD, NRM, false);           \
+    } while (0)
     const bool upd = qprev != nullptr, nrm = q == nullptr;
     if (ctx->dtype == B2K_F64) {
         if (upd && nrm) LAUNCH(double, true, true);
@@ -718,18 +1087,21 @@ int32_t b2k_enqueue_dot(b2k_ctx* ctx, const void* q, void* x, int64_t n, const v
         else LAUNCH(float, false, false);
     }
 #undef LAUNCH
+#undef LAUNCH_S
     B2K_LAUNCH_CHECK(ctx);
     return B2K_OK;
 }
 
 int32_t b2k_enqueue_axpy_dev(b2k_ctx* ctx, void* x, const void* q, int s_slot, int64_t n) {
     const int grid = grid_for(ctx, n, 8);
-    if (ctx->dtype == B2K_F64)
-        k_axpy_dev<double><<<grid, BT, 0, ctx->stream>>>((double*)x, (const double*)q,
-                                                         ctx->d_res + s_slot, n);
-    else
-        k_axpy_dev<float><<<grid, BT, 0, ctx->stream>>>((float*)x, (const float*)q,
-                                                        ctx->d_res + s_slot, n);
+    const int* st = ctx->dot_stop;
+    if (ctx->dtype == B2K_F64) {
+        if (st) k_axpy_dev<double, true><<<grid, BT, 0, ctx->stream>>>((double*)x, (const double*)q, ctx->d_res + s_slot, n, st);
+        else k_axpy_dev<double><<<grid, BT, 0, ctx->stream>>>((double*)x, (const double*)q, ctx->d_res + s_slot, n, st);
+    } else {
+        if (st) k_axpy_dev<float, true><<<grid, BT, 0, ctx->stream>>>((float*)x, (const float*)q, ctx->d_res + s_slot, n, st);
+        else k_axpy_dev<float><<<grid, BT, 0, ctx->stream>>>((float*)x, (const float*)q, ctx->d_res + s_slot, n, st);
+    }
     B2K_LAUNCH_CHECK(ctx);
     return B2K_OK;
 }

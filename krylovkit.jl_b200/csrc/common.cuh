@@ -55,6 +55,8 @@ struct b2k_ctx {
     int32_t num_sms = 0;
     size_t  l2_persist_bytes = 0;   // persisting-L2 carve-out (0 = unavailable)
     int     dot_hints = 0;          // set by the MGS sweep: its k_dot launches carry L2 eviction-priority hints
+    const int* dot_stop = nullptr;  // set by b2k_lsmr_chain around its MGS sweeps: k_dot / k_axpy_dev do nothing once
+                                    // this device flag is raised (null: the instances without the check)
     unsigned long long* d_trace = nullptr;   // b2k_debug_trace: [0] event count, then (globaltimer ns, code) pairs
     size_t  l2_window_max = 0;      // max access-policy window
     cudaStream_t stream = nullptr;
@@ -69,7 +71,8 @@ struct b2k_ctx {
     double*   d_coef   = nullptr;   // coefficients uploaded from host
     double*   h_coef   = nullptr;   // pinned staging
     unsigned* d_sync   = nullptr;   // [0] ticket, [1] grid barrier counter, ... (B2K_SYNC_*)
-    double*   d_steps  = nullptr;   // (B2K_MAX_CHAIN + 1) step records of B2K_REC doubles
+    double*   d_steps  = nullptr;   // 2 (B2K_MAX_CHAIN + 1) step records of B2K_REC doubles (the LSMR chain uses two
+                                    // per iteration)
     double*   d_blk    = nullptr;   // block path (block.cu): coefficient blocks H1 | H2 | Gram
     double*   d_blkpart = nullptr;  // block path: per-CTA partials
     cudaEvent_t ev_coef = nullptr;  // guards reuse of the pinned staging buffers
@@ -217,6 +220,37 @@ struct SpmvFuse {
     const double* acoef;
     double* nrm_out;
 };
+
+// LSMR chain (b2k_lsmr_chain, basis.cu; kernels in blas1.cu).  Device state, LS_NSTATE doubles at d_steps:
+//   [0, LS_NIO)  the state handed in and out: alpha, beta, alphabar, rho, rhobar, cbar, sbar, theta, zetabar, lambda
+//   LS_INVA      scale of the stored v operand (1 on entry: v normalised; 1/alpha once v~ is left unnormalised)
+//   LS_INVB      scale of the stored u (1 on entry; 1/beta after the m-side step)
+//   LS_G, LS_CZ  g and zeta/(rho rhobar) of the last recurrence: the h-bar, x, Ah-bar, r updates still pending
+//   LS_BSKIP     beta <= tol in the last iteration (A' product skipped, u left unnormalised, alpha and v kept)
+//   LS_ASKIP     alpha <= tol in the last iteration (v left unnormalised, not pushed into the ring)
+//   LS_DONE      iterations this call has completed; LS_FIN: 5 doubles of scratch for the Gram-Schmidt finaliser
+// followed by LS_REC doubles per iteration (two B2K_REC records).
+enum { LS_ALPHA = 0, LS_BETA, LS_ALPHABAR, LS_RHO, LS_RHOBAR, LS_CBAR, LS_SBAR, LS_THETA, LS_ZETABAR, LS_LAM,
+       LS_NIO, LS_INVA = LS_NIO, LS_INVB, LS_G, LS_CZ, LS_BSKIP, LS_ASKIP, LS_DONE, LS_FIN = 24, LS_NSTATE = 32 };
+constexpr int LS_REC = 2 * B2K_REC;
+constexpr int LS_MAXRING = 128;             // ring columns a chained call takes
+constexpr int B2K_SYNC_SKIP = 6;            // d_sync slot: the LSMR chain's A'-side skip flag
+struct LsmrDev {
+    double* st;
+    double* rec0;
+    int* stop;               // raised by the recurrence: every later launch of the call does nothing
+    int* skip;               // stop, or beta <= tol: the A' SpMV and the reorthogonalisation do nothing
+    double tol;
+    int iter0;               // iterations completed before the call (v_{iter0+1} sits in ring slot iter0 % nring)
+    int nring;
+    void* ring[LS_MAXRING];  // read by the flush launch only
+};
+int32_t b2k_lsmr_enqueue_m(b2k_ctx* ctx, int64_t m, void* r, void* Ah, void* Ahbar, void* u, const void* Av,
+                           bool pend, bool flush, const LsmrDev& d);
+int32_t b2k_lsmr_enqueue_n(b2k_ctx* ctx, int64_t n, void* x, void* h, void* hbar, void* P, void* Q, bool swap,
+                           bool pend, bool norm, const LsmrDev& d);
+int32_t b2k_lsmr_enqueue_alpha(b2k_ctx* ctx, int64_t n, const void* Q, const LsmrDev& d);
+int32_t b2k_lsmr_enqueue_flush_n(b2k_ctx* ctx, int64_t n, void* x, void* h, void* hbar, void* spare, const LsmrDev& d);
 
 int32_t b2k_enqueue_apply(b2k_ctx* ctx, const b2k_op* op, const VecRef& x, const VecRef& y,
                           double a0, double a1, bool shifted, const VecRef* dotv, int dot_slot);

@@ -241,8 +241,8 @@ static int32_t ctx_create_common(b2k_ctx** out, int32_t device, int64_t n_local,
     CK(b2k_hmalloc((void**)&ctx->h_res, sizeof(double) * B2K_RES_DOUBLES));
     CK(B2K_DMALLOC(&ctx->d_coef, sizeof(double) * B2K_COEF_DOUBLES));
     CK(b2k_hmalloc((void**)&ctx->h_coef, sizeof(double) * B2K_COEF_DOUBLES));
-    CK(B2K_DMALLOC(&ctx->d_steps, sizeof(double) * B2K_REC * (B2K_MAX_CHAIN + 1)));
-    CK(cudaMemsetAsync(ctx->d_steps, 0, sizeof(double) * B2K_REC * (B2K_MAX_CHAIN + 1), ctx->stream));
+    CK(B2K_DMALLOC(&ctx->d_steps, sizeof(double) * 2 * B2K_REC * (B2K_MAX_CHAIN + 1)));
+    CK(cudaMemsetAsync(ctx->d_steps, 0, sizeof(double) * 2 * B2K_REC * (B2K_MAX_CHAIN + 1), ctx->stream));
     CK(B2K_DMALLOC(&ctx->d_blk, sizeof(double) * (2 * B2K_BLK_HCAP + 64)));
     CK(B2K_DMALLOC(&ctx->d_blkpart, sizeof(double) * (size_t)B2K_MAX_GRID * B2K_BLK_PART));
     CK(B2K_DMALLOC(&ctx->d_sync, sizeof(unsigned) * 64));

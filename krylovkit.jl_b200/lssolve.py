@@ -4,18 +4,30 @@ min_x ‖b − A x‖² + λ²‖x‖² by Golub-Kahan bidiagonalisation; every 
 VectorInterface call on device vectors, the scalar rotations stay on the host.  The operator is
 anything `apply_normal` / `apply_adjoint` accept: a B200Dense, a pair (A, Aᵀ) of B200CSR
 operators (rectangular ones carry `space_in` / `space_out`), or a callable f(x, flag).
+
+A B200CSR itself is accepted too: Aᵀ is built on the device for the call, and on one GPU the
+iterations are chained on the device (b2k_lsmr_chain, LSMR_CHAIN_LEN per host round trip) when
+the reorthogonalisation can be: krylovdim <= 1, or MGS, MGS2, CGS2 or the flagged MGS2B.
 """
 from __future__ import annotations
 
+import ctypes as C
 import math
 import warnings
 
 import numpy as np
 
+from . import _lib as L
+from ._lib import B200Error
 from .algorithms import ConvergenceInfo, LSMR, WARN_LEVEL
 from .operators import B200CSR, B200Dense, apply_adjoint, apply_normal
 from .orthonormal import OrthonormalBasis, orthogonalize_
-from .vectors import B200Context, B200Vec
+from .vectors import B200Context, B200Vec, handles
+
+USE_LSMR_CHAIN = True    # b2k_lsmr_chain: four launches per iteration (+ the reorthogonalisation), one round trip
+LSMR_CHAIN_LEN = 32      # per LSMR_CHAIN_LEN iterations
+_FORMS = ("lssolve takes a B200CSR (single-GPU context, stored matrix) or a scipy sparse matrix, a dense numpy "
+          "matrix or B200Dense, an (A, At) tuple of operators, or a callable f(x, adjoint)")
 
 
 def lssolve(A, b, alg: LSMR | None = None, lam: float = 0.0, atol: float | None = None,
@@ -26,6 +38,8 @@ def lssolve(A, b, alg: LSMR | None = None, lam: float = 0.0, atol: float | None 
     if alg is None:
         alg = LSMR(**kwargs)
     if isinstance(b, B200Vec):
+        if isinstance(A, B200CSR):
+            return _lssolve_csr(A, b, alg, lam, atol, rtol)
         if atol is not None or rtol is not None:
             alg = _retol(alg, max(atol or 0.0, (rtol or 0.0) * apply_adjoint(A, b).norm()))
         return _lsmr(A, b, alg, lam)
@@ -48,12 +62,40 @@ def lssolve(A, b, alg: LSMR | None = None, lam: float = 0.0, atol: float | None 
         ctx.close()
 
 
+def _lssolve_csr(A: B200CSR, b: B200Vec, alg: LSMR, lam: float, atol, rtol):
+    """lssolve on a device CSR matrix: Aᵀ is built on the device (B200CSR.transpose()) and freed before returning."""
+    ctx = b.ctx
+    if ctx.nranks > 1:
+        raise B200Error(f"lssolve: row-sharded contexts are not supported; {_FORMS}")
+    nr, nc, nnz, kind = C.c_int64(), C.c_int64(), C.c_int64(), C.c_int32()
+    ctx.check(ctx.lib.b2k_op_info(A.h, C.byref(nr), C.byref(nc), C.byref(nnz), C.byref(kind)))
+    if kind.value == 2:
+        raise B200Error(f"lssolve: a matrix-free stencil has no transpose; {_FORMS}")
+    if kind.value != 0:
+        raise B200Error(f"lssolve: the operator is not a stored CSR matrix; {_FORMS}")
+    if not A._explicit_spaces and A.n_rows != A.n_cols:
+        raise ValueError("lssolve: a rectangular B200CSR must carry its spaces (A.with_spaces(space_in, space_out))")
+    At = A.transpose()
+    try:
+        op = (A, At)
+        if atol is not None or rtol is not None:
+            alg = _retol(alg, max(atol or 0.0, (rtol or 0.0) * apply_adjoint(op, b).norm()))
+        K = alg.krylovdim
+        # the library refuses what it cannot chain (B2K_ENOTSUP, nothing written): the loop then runs literally
+        chain = USE_LSMR_CHAIN and (K <= 1 or alg.orth.tag in (L.MGS, L.MGS2, L.CGS2, L.MGS2B))
+        return _lsmr(op, b, alg, lam, chain=chain)
+    finally:
+        At.free()
+
+
 def _retol(alg: LSMR, tol: float) -> LSMR:
     return LSMR(orth=alg.orth, maxiter=alg.maxiter, krylovdim=alg.krylovdim, tol=tol, verbosity=alg.verbosity)
 
 
-def _lsmr(operator, b: B200Vec, alg: LSMR, lam: float):
-    """lssolve(operator, b, alg::LSMR, λ) — lsmr.jl:1-162."""
+def _lsmr(operator, b: B200Vec, alg: LSMR, lam: float, chain: bool = False):
+    """lssolve(operator, b, alg::LSMR, λ) — lsmr.jl:1-162.  chain (operator = (A, Aᵀ) of stored CSR matrices on
+    one GPU): the iterations run LSMR_CHAIN_LEN at a time in b2k_lsmr_chain, and a beta or alpha breakdown hands
+    the state back to the loop below, which completes the solve as the reference does."""
     u = b.copy()
     v = apply_adjoint(operator, b)
     beta = u.norm()
@@ -81,6 +123,57 @@ def _lsmr(operator, b: B200Vec, alg: LSMR, lam: float):
     maxiter, tol = alg.maxiter, alg.tol
     if abszetabar < tol:
         return x, ConvergenceInfo(1, r, abszetabar, numiter, numops)
+
+    if chain:
+        ctx = b.ctx
+        R = max(K, 1)
+        ring = [v] + [ctx.empty(v.space) for _ in range(R - 1)]
+        spare, Av = ctx.empty(v.space), ctx.empty(u.space)
+        ring_h = handles(ring)
+        state = (C.c_double * 10)()
+        state_out = (C.c_double * 10)()
+        rec = np.zeros((LSMR_CHAIN_LEN, 16))
+        done = C.c_int32()
+        while True:
+            nsteps = max(1, min(LSMR_CHAIN_LEN, maxiter - numiter))
+            state[:] = [alpha, beta, alphabar, rho, rhobar, cbar, sbar, theta, zetabar, lam]
+            status = ctx.lib.b2k_lsmr_chain(
+                ctx.h, operator[0].h, operator[1].h, x.handle, h.handle, hbar.handle, r.handle, Ah.handle,
+                Ahbar.handle, u.handle, Av.handle, ring_h, K, spare.handle, alg.orth.tag, numiter, state, tol,
+                nsteps, rec.ctypes.data_as(C.POINTER(C.c_double)), state_out, C.byref(done))
+            if status == L.ENOTSUP and numiter == 0:
+                # e.g. more ring columns than the cooperative sweep holds, or that sweep switched off
+                V = OrthonormalBasis([v])
+                del ring, spare, Av
+                break
+            ctx.check(status)
+            d = done.value
+            numiter += d
+            numops += d + int(rec[:d, 8].sum())
+            alpha, beta, alphabar, rho, rhobar, cbar, sbar, theta, zetabar = list(state_out)[:9]
+            abszetabar = rec[d - 1, 6]
+            code = int(rec[d - 1, 7])
+            if code == 1:
+                return x, ConvergenceInfo(1, r, abszetabar, numiter, numops)
+            if code == 0 and numiter < maxiter:
+                continue
+            # hand the loop's state to the literal iterations below (include/b200krylov.h: where v is)
+            if code == 2:
+                v = ring[(numiter - 1) % R]
+                V = OrthonormalBasis(ring[:min(K, numiter)] if K > 1 else ring[:1])
+            elif code == 3:
+                v = spare
+                V = OrthonormalBasis(ring[:min(K, numiter)] if K > 1 else ring[:1])
+            else:
+                v = ring[numiter % R]
+                V = OrthonormalBasis(ring[:min(K, numiter + 1)] if K > 1 else ring[:1])
+            del ring, spare, Av
+            if numiter >= maxiter:
+                if alg.verbosity >= WARN_LEVEL:
+                    warnings.warn(f"LSMR lssolve stopped without converging after {numiter} iterations: "
+                                  f"normres = {abszetabar}, numops = {numops}")
+                return x, ConvergenceInfo(0, r, abszetabar, numiter, numops)
+            break
 
     while True:
         numiter += 1

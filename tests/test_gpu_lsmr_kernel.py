@@ -1,0 +1,167 @@
+"""GPU tests of b2k_lsmr_chain against the fma-order restatement of tests/lsmr_restate.py: one chained iteration,
+bit for bit — every vector, the ring, the record and the state — in Float64 and Float32, with and without lambda,
+without reorthogonalisation and with a ring of 5 under MGS, MGS2 and CGS2; the beta and alpha sums against the
+restated CTA-ordered sums; and the breakdown stop codes 2 (beta <= tol) and 3 (alpha <= tol) on the device."""
+import contextlib
+import ctypes as C
+
+import numpy as np
+import pytest
+import scipy.sparse as sp
+
+pytestmark = pytest.mark.gpu
+
+import krylovkit_jl_b200 as kk
+from krylovkit_jl_b200 import _lib as L
+from test_gpu_blas1 import fma  # noqa: F401  (fixture: correctly rounded fused multiply-add on the host)
+
+import lsmr_restate as LR
+
+f64, f32 = np.float64, np.float32
+
+
+def nsm():
+    import torch
+    return torch.cuda.get_device_properties(0).multi_processor_count
+
+
+@contextlib.contextmanager
+def plain_kernel():
+    """the plain TMA SpMV kernel (the compact copy off), the one spmv_restate's "pipe" rows restate"""
+    lib = L.load()
+    lib.b2k_debug_set_csr_compact(0)
+    try:
+        yield
+    finally:
+        lib.b2k_debug_set_csr_compact(1)
+
+
+def same(a, b):
+    a, b = np.asarray(a), np.asarray(b)
+    return a.dtype == b.dtype and a.shape == b.shape and a.tobytes() == b.tobytes()
+
+
+def rect(m, n, seed):
+    A = (sp.random(m, n, density=0.01, random_state=seed) + sp.eye(m, n)).tocsr()
+    A.sort_indices()
+    return A
+
+
+class Setup:
+    def __init__(self, A, dt, K, seed=5):
+        self.A, self.dt, self.K, self.R = A, dt, K, max(K, 1)
+        m, n = A.shape
+        self.ctx = kk.B200Context(m, 16, dtype=dt)
+        self.sv = self.ctx.add_space(n, self.R + 12, sharded=False)
+        self.op = kk.B200CSR.from_scipy(self.ctx, A.astype(dt)).with_spaces(self.sv, 0)
+        self.opt = self.op.transpose()
+        rng = np.random.default_rng(seed)
+        self.host = {k: rng.standard_normal(n).astype(dt) for k in ("x", "h", "hbar")}
+        self.host.update({k: rng.standard_normal(m).astype(dt) for k in ("r", "Ah", "Ahbar", "u")})
+        Q = np.linalg.qr(rng.standard_normal((n, self.R)))[0].astype(dt)
+        self.ring = [Q[:, j].copy() for j in range(self.R)]
+
+    def upload(self, host=None, ring=None):
+        host, ring = host or self.host, ring or self.ring
+        c = self.ctx
+        self.d = {k: c.from_host(v, self.sv if len(v) == self.A.shape[1] else 0) for k, v in host.items()}
+        self.d["av"] = c.zeros()
+        self.dring = [c.from_host(q, self.sv) for q in ring]
+        self.dspare = c.zeros(self.sv)
+
+    def call(self, st, tol, iter0, nsteps, alg):
+        rec, done = np.zeros((nsteps, 16)), C.c_int32(-1)
+        sin, sout = (C.c_double * 10)(*st), (C.c_double * 10)()
+        rh = (L.c_vec * self.R)(*[q.handle for q in self.dring])
+        d = self.d
+        s = self.ctx.lib.b2k_lsmr_chain(self.ctx.h, self.op.h, self.opt.h, d["x"].handle, d["h"].handle,
+                                        d["hbar"].handle, d["r"].handle, d["Ah"].handle, d["Ahbar"].handle,
+                                        d["u"].handle, d["av"].handle, rh, self.K, self.dspare.handle, alg, iter0,
+                                        sin, tol, nsteps, rec.ctypes.data_as(C.POINTER(C.c_double)), sout,
+                                        C.byref(done))
+        return s, rec[:max(done.value, 0)], list(sout)
+
+    def close(self):
+        self.opt.free()
+        self.op.free()
+        self.ctx.close()
+
+
+STATE = [1.3, 0.7, 0.9, 1.1, 1.4, 0.8, 0.6, 0.35, 0.5]
+
+
+@pytest.mark.parametrize("dt", [f64, f32], ids=["f64", "f32"])
+@pytest.mark.parametrize("lam", [0.0, 0.3])
+@pytest.mark.parametrize("K,alg", [(1, L.MGS), (5, L.MGS), (5, L.MGS2), (5, L.CGS2)], ids=["k1", "mgs", "mgs2", "cgs2"])
+def test_one_iteration_bit_for_bit(fma, dt, lam, K, alg):
+    A = rect(3000, 800, 4)
+    s = Setup(A, dt, K)
+    try:
+        k = 8                                        # the ring is full: the sweep covers all 5 slots, v_8 in slot 2
+        st = STATE + [lam]
+        s.upload()
+        with plain_kernel():
+            status, rec, sout = s.call(st, 0.0, k - 1, 1, alg)
+        assert status == L.OK and len(rec) == 1
+        At = A.T.tocsr()
+        At.sort_indices()
+        out, ring, spare, a_sum, b_sum, st2, rrec = LR.iteration(fma, dt, A.astype(dt), At.astype(dt), st, s.host,
+                                                                 s.ring, K, alg, 0.0, nsm(), k, alpha_dev=rec[0, 0],
+                                                                 beta_dev=rec[0, 1])
+        # the CTA-ordered sums
+        assert same(f64(rec[0, 1]), f64(b_sum)), (rec[0, 1], b_sum)
+        assert same(f64(rec[0, 0]), f64(a_sum)), (rec[0, 0], a_sum)
+        # the recurrence and its record
+        assert same(rec[0, :14], np.array(rrec[:14])), (rec[0], rrec)
+        assert same(np.array(sout), np.array(st2))
+        # every vector and the ring
+        for key in ("x", "h", "hbar", "r", "Ah", "Ahbar", "u"):
+            assert same(s.d[key].to_host(), out[key]), key
+        for j in range(s.R):
+            assert same(s.dring[j].to_host(), ring[j]), j
+    finally:
+        s.close()
+
+
+def breakdown_problem(kind, seed=7):
+    """three distinct singular values; b in the range (the u side runs out: beta <= tol), or with a part orthogonal
+    to it (the v side runs out: alpha <= tol).  b is large, so |zetabar| is still above tol when that happens."""
+    rng = np.random.default_rng(seed)
+    m, n = 400, 120
+    U, _ = np.linalg.qr(rng.standard_normal((m, n)))
+    V, _ = np.linalg.qr(rng.standard_normal((n, n)))
+    A = sp.csr_matrix(U @ np.diag(np.repeat([3.0, 2.0, 1.0], n // 3)) @ V.T)
+    A.sort_indices()
+    b = A @ rng.standard_normal(n)
+    if kind == "alpha":
+        w = rng.standard_normal(m)
+        b = b + (w - U @ (U.T @ w))
+    return A, 1e6 * b
+
+
+@pytest.mark.parametrize("kind,code", [("beta", 2), ("alpha", 3)])
+@pytest.mark.parametrize("K,alg", [(1, L.MGS), (4, L.MGS), (4, L.CGS2)], ids=["k1", "mgs", "cgs2"])
+def test_breakdown_stop_codes(kind, code, K, alg):
+    A, b = breakdown_problem(kind)
+    s = Setup(A, f64, K)
+    try:
+        beta = float(np.linalg.norm(b))
+        u = b / beta
+        v = (A.T @ b) / beta
+        alpha = float(np.linalg.norm(v))
+        v = v / alpha
+        n, m = A.shape[1], A.shape[0]
+        host = {"x": np.zeros(n), "h": v.copy(), "hbar": np.zeros(n), "r": b.copy(), "Ah": np.zeros(m),
+                "Ahbar": np.zeros(m), "u": u}
+        ring = [v] + [np.zeros(n) for _ in range(s.R - 1)]
+        s.upload(host, ring)
+        status, rec, sout = s.call([alpha, beta, alpha, 1.0, 1.0, 1.0, 0.0, 0.0, alpha * beta, 0.0], 1e-8, 0, 20,
+                                   alg)
+        assert status == L.OK
+        assert rec[-1, 7] == code and len(rec) < 20
+        assert rec[-1, 6] > 1e-8                     # not converged: the driver continues with the literal loop
+        assert rec[-1, 8] == (0.0 if code == 2 else 1.0)
+        if code == 3:                                # v stays unnormalised in the spare column, the ring untouched
+            assert np.linalg.norm(s.dspare.to_host()) <= 1e-8
+    finally:
+        s.close()
