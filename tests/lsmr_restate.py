@@ -35,37 +35,94 @@ VEC = {f64: 2, f32: 4}
 
 
 def _hyp(a, b):
-    return math.sqrt(a * a + b * b)
+    return np.sqrt(a * a + b * b)
 
 
 def lsmr_scalars(st, alpha, beta, bskip, tol):
-    """The device recurrence (blas1.cu::lsmr_recurrence) in plain double arithmetic: st = the 10-double state of the
-    iteration's start; alpha, beta of this iteration.  Returns (new state, record of 16)."""
-    _, _, alphabar, rhoold, rhobarold, cbar0, sbar0, _, zetabar0, lam = st
-    alphahat = _hyp(alphabar, lam)
-    rho = _hyp(alphahat, beta)
-    c, s = alphahat / rho, beta / rho
-    theta = s * alpha
-    alphabar = c * alpha
-    thetabar = sbar0 * rho
-    cbarrho = cbar0 * rho
-    rhobar = _hyp(cbarrho, theta)
-    cbar, sbar = cbarrho / rhobar, theta / rhobar
-    zeta = cbar * zetabar0
-    zetabar = -sbar * zetabar0
-    g = (-thetabar * rho) / (rhoold * rhobarold)
-    cz = zeta / (rho * rhobar)
+    """The device recurrence (blas1.cu::lsmr_recurrence) in np.float64 arithmetic, every operation rounded on its own
+    and non-finite values carried through rather than raised (a division by zero is the code-4 path): st = the
+    10-double state of the iteration's start; alpha, beta of this iteration.  Returns (new state, record of 16)."""
+    _, _, alphabar, rhoold, rhobarold, cbar0, sbar0, _, zetabar0, lam = (f64(t) for t in st)
+    alpha, beta = f64(alpha), f64(beta)
+    with np.errstate(all="ignore"):
+        alphahat = _hyp(alphabar, lam)
+        rho = _hyp(alphahat, beta)
+        c, s = alphahat / rho, beta / rho
+        theta = s * alpha
+        alphabar = c * alpha
+        thetabar = sbar0 * rho
+        cbarrho = cbar0 * rho
+        rhobar = _hyp(cbarrho, theta)
+        cbar, sbar = cbarrho / rhobar, theta / rhobar
+        zeta = cbar * zetabar0
+        zetabar = -sbar * zetabar0
+        g = (-thetabar * rho) / (rhoold * rhobarold)
+        cz = zeta / (rho * rhobar)
     askip = not bskip and not alpha > tol
-    fin = all(math.isfinite(t) for t in (alpha, beta, rho, rhobar, g, cz, zetabar))
+    fin = all(np.isfinite(t) for t in (alpha, beta, rho, rhobar, g, cz, zetabar))
     code = 1.0 if abs(zetabar) <= tol else 2.0 if bskip else 3.0 if askip else 4.0 if not fin else 0.0
     rec = [alpha, beta, rho, rhobar, theta, zeta, abs(zetabar), code, 0.0 if bskip else 1.0, alphabar, cbar, sbar, g,
            cz, 0.0, 0.0]
-    return [alpha, beta, alphabar, rho, rhobar, cbar, sbar, theta, zetabar, lam], rec
+    return [alpha, beta, alphabar, rho, rhobar, cbar, sbar, theta, zetabar, lam], [f64(t) for t in rec]
 
 
 def grid_for(n, per_thread, nsm):
     want = max(1, -(-n // (BT * per_thread)))
     return int(min(want, CTAS_PER_SM * nsm))
+
+
+# Edge lengths of the streaming kernels of blas1.cu.  A kernel launches grid_for(n, per_thread) CTAs of BT threads;
+# thread t visits the 128-bit vectors t, t + BT G, t + 2 BT G, ... (G the grid) in trips of `unroll` slots
+# (B2K_TRIP(unroll)), and CTA 0 takes the n % V tail elements.
+SMALL = (1, 2, 3, "V-1", "V+1", 255, 257)
+
+
+def cap_size(per_thread, nsm):
+    """the largest n whose grid is exactly 4 SMs CTAs without clamping, tail empty in both types"""
+    return per_thread * BT * CTAS_PER_SM * nsm
+
+
+def trips_size(dt, unroll, nsm):
+    """at the capped grid: 2 unroll + 1 full vectors per thread plus one more for the first half of the threads (three
+    trips, the last one's second slot live for half of them), and a tail of V - 1 elements"""
+    T = BT * CTAS_PER_SM * nsm
+    return VEC[dt] * ((2 * unroll + 1) * T + T // 2) + VEC[dt] - 1
+
+
+def edge_size(name, dt, per_thread, unroll, nsm):
+    if name == "cap":
+        return cap_size(per_thread, nsm)
+    if name == "trips":
+        return trips_size(dt, unroll, nsm)
+    if name == "V-1":
+        return VEC[dt] - 1
+    if name == "V+1":
+        return VEC[dt] + 1
+    return name
+
+
+def trip_profile(n, dt, per_thread, unroll, nsm):
+    """what a length does to a streaming kernel: (grid, capped, most trips of a thread, the second slot of the last
+    trip live for some threads but not all, tail length)"""
+    V = VEC[dt]
+    g = grid_for(n, per_thread, nsm)
+    T = g * BT
+    nv = n // V
+    t = np.arange(T)
+    cnt = np.where(t < nv, -(-(nv - t) // T), 0)                 # vectors of thread t
+    trips = -(-cnt // unroll)
+    in_last = np.where(cnt > 0, cnt - unroll * (trips - 1), 0)   # live slots of its last trip
+    partial = 0 < int(np.count_nonzero(in_last >= 2)) < int(np.count_nonzero(cnt))
+    return g, g == CTAS_PER_SM * nsm, int(trips.max(initial=0)), partial, n - nv * V
+
+
+def check_edge(name, n, dt, per_thread, unroll, nsm):
+    """assert that n has the property its name promises for this kernel"""
+    g, capped, trips, partial, tail = trip_profile(n, dt, per_thread, unroll, nsm)
+    if name == "cap":
+        assert capped and tail == 0 and n == BT * per_thread * g, (name, n)
+    elif name == "trips":
+        assert capped and trips >= 3 and partial and tail > 0, (name, n, trips, partial, tail)
 
 
 def thread_dots(fma, dt, a, b, grid):
@@ -124,7 +181,12 @@ def iteration(fma, dt, A, At, st, vec, ring, K, alg, tol, nsm, k, alpha_dev=None
     """One call of one iteration (the first of the call, so nothing pending on entry).  vec: dict of host vectors
     x, h, hbar, r, Ah, Ahbar, u; ring: list of R host columns (v_k in slot (k - 1) % R).  alpha_dev / beta_dev:
     take these for the vectors (the sums are then checked on their own).  Returns (vectors, ring, spare, alpha,
-    beta, state, record)."""
+    beta, state, record).  Non-finite scalars (a code-4 stop) propagate into the vectors as they do on the device."""
+    with np.errstate(all="ignore"):
+        return _iteration(fma, dt, A, At, st, vec, ring, K, alg, tol, nsm, k, alpha_dev, beta_dev)
+
+
+def _iteration(fma, dt, A, At, st, vec, ring, K, alg, tol, nsm, k, alpha_dev, beta_dev):
     import krylovkit_jl_b200._lib as L
     Rn = max(K, 1)
     m, n = A.shape
