@@ -1784,9 +1784,23 @@ extern "C" int32_t b2k_lanczos_expand(b2k_ctx* ctx, const b2k_op* op, const b2k_
 
     // MGS family (lanczos.jl:304-312, 325-338, 357-376): w = A v ; w -= beta v_prev ;
     // alpha = <v, w> ; w -= alpha v ; [second sweep over all of V]
-    B2K_TRY(b2k_enqueue_apply(ctx, op, rv, rw, 0.0, 1.0, false, nullptr, -1));
-    B2K_TRY(b2k_vec_axpby(ctx, w, cols[k - 1], -beta_old, 1.0));
-    B2K_TRY(b2k_enqueue_dot(ctx, rv.ptr, rw.ptr, pn.n, nullptr, -1, S_A0, -1));
+    int32_t op_kind = -1;
+    B2K_TRY(b2k_op_info(op, nullptr, nullptr, nullptr, &op_kind));
+    if (alg == B2K_MGS2B && op_kind != 1) {
+        // alpha = <v, A v - beta v_prev> fused into the SpMV epilogue (dot_sub_vec), the order of the chained step
+        // (lanczos_chain), so that a chained batch and these steps give the same bits
+        SpmvFuse fz;
+        memset(&fz, 0, sizeof(fz));
+        fz.dot_sub_vec = vprev.ptr;
+        fz.dot_sub_scale = ctx->d_coef;
+        B2K_TRY(b2k_put_coef(ctx, &beta_old, 1, 0));
+        B2K_TRY(b2k_enqueue_apply_fused(ctx, op, rv, rw, 0.0, 1.0, false, &rv, ctx->d_res + S_A0, &fz));
+        B2K_TRY(b2k_vec_axpby(ctx, w, cols[k - 1], -beta_old, 1.0));
+    } else {
+        B2K_TRY(b2k_enqueue_apply(ctx, op, rv, rw, 0.0, 1.0, false, nullptr, -1));
+        B2K_TRY(b2k_vec_axpby(ctx, w, cols[k - 1], -beta_old, 1.0));
+        B2K_TRY(b2k_enqueue_dot(ctx, rv.ptr, rw.ptr, pn.n, nullptr, -1, S_A0, -1));
+    }
     B2K_TRY(b2k_allreduce(ctx, ctx->d_res + S_A0, 1, pn.sharded));
     B2K_TRY(b2k_enqueue_axpy_dev(ctx, rw.ptr, rv.ptr, S_A0, pn.n));
     double alpha = 0.0, beta = 0.0;
@@ -1852,7 +1866,9 @@ extern "C" int32_t b2k_lanczos_expand(b2k_ctx* ctx, const b2k_op* op, const b2k_
 // The reference looks at β after every step (eigsolve/lanczos.jl:45: `while K < krylovdim && β > tol`), so do
 // the kernels: a record with β <= tol raises a device flag and everything enqueued behind it does nothing.  The
 // host reads all records with ONE synchronisation at the end of the batch and commits the steps up to the
-// first β <= tol — same α, β, V, r as stepping one at a time, bit for bit (same kernels, same operand bits).
+// first β <= tol — same α, β, V, r as stepping one at a time, bit for bit (same kernels, same operand bits).  The
+// flagged ModifiedGramSchmidt2Blocked chains too: its α₀ = <v, A v − β v₋> comes from the SpMV epilogue
+// (dot_sub_vec) in the chain and in the synchronous step (b2k_lanczos_expand) alike, on CSR and stencil operators.
 bool g_use_chain = true;
 
 bool chain_ok(const b2k_ctx* ctx, const b2k_op* op, const b2k_vec* cols, int32_t k, int32_t nsteps, int32_t alg,

@@ -475,8 +475,9 @@ extern "C" int32_t b2k_vec_zero(b2k_ctx* ctx, b2k_vec v) {
 
 int32_t b2k_allreduce(b2k_ctx* ctx, double* dptr, int32_t count, int32_t sharded) {
     if (ctx->nranks > 1 && sharded) {
-        if (b2k_peer_ok(ctx) && count <= PEER_SLOT) return b2k_peer_allreduce(ctx, dptr, count);
-        if (b2k_peer_ok(ctx) && !b2k_has_nccl(ctx)) {          // peer-only transport: in slot-sized pieces
+        // over the peer window every count is the rank-order fold, in slot-sized pieces, whether or not the
+        // context also has an NCCL communicator
+        if (b2k_peer_ok(ctx)) {
             for (int32_t off = 0; off < count; off += PEER_SLOT)
                 B2K_TRY(b2k_peer_allreduce(ctx, dptr + off, std::min<int32_t>(PEER_SLOT, count - off)));
             return B2K_OK;

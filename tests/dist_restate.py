@@ -151,3 +151,263 @@ def lanczos_step(fma, dt, sizes, V, r, beta_old, csr, spmv_kernel, spmv_grids, n
         n2s.append(ts.normsum(ts.norm_partials(w, nsm, fma)))
     n2 = float(fold(n2s))
     return out, v, alpha0, alpha0 + float(h[-1]), float(np.sqrt(n2)), n2
+
+
+# ------------------------------------------------------------------------------ the other sharded entry points ----
+#
+# Every sharded entry point below sums across ranks only through b2k_allreduce, so each restatement is rank p's
+# single-GPU order on its row slice (G_p = the local grid), folded where the device all-reduces:
+#   b2k_basis_project     h = fold(tsk_restate.project(Q_p, x_p)), per pass of kcap columns the colsum of that pass,
+#                         one all-reduce of all k doubles (slot-sized pieces past PEER_SLOT = 1024);
+#   classical pass        cgs_pass_unfused_t: h = that fold, v_p = update(Q_p, v_p, coefs(h, -1)), ||v||^2 =
+#                         fold(normsum(norm_partials(v_p))); fused_ok() is false on a sharded panel, so CGS, CGS2,
+#                         CGSIR and MGS2B always take it;
+#   k_dot                 s = fold(lsmr_restate.blas1_sum(a_p, b_p, grid_for(n_p, 8))): inner, norm, every ||v||^2
+#                         of the MGS family and the vector orthogonalizer, and each s_j of mgs_sweep, which is folded
+#                         before the next pipelined k_dot subtracts it (x = fma(-T(s_{j-1}), q_{j-1}, x));
+#   CG / BiCGStab steps   the SpMV's fused dot (this module's spmv) and the k_cg_xr / k_bicg_s / k_bicg_xr sums, the
+#                         latter in blas1_sum's order on grid_for(n_p, 8);
+#   the IR loops          decide on the folded norms only, so every rank runs the same number of passes.
+# A replicated space (sharded = 0) is summed on no rank: every rank's value is the one-rank restatement of the full
+# vectors.
+
+import math  # noqa: E402
+
+import lsmr_restate as LS  # noqa: E402
+
+EPS = {f64: 2.0 ** -52, np.float32: 2.0 ** -23}
+
+
+def rows(sizes, a):
+    """the rank slices of a global vector or row panel"""
+    off = offsets(sizes)
+    return [a[off[p]:off[p + 1]] for p in range(len(sizes))]
+
+
+def dot(fma, dt, sizes, a, b, nsm):
+    """k_dot on the shards, all-reduced: the fold of every rank's blas1_sum on its grid_for(n_p, 8)"""
+    return float(fold([LS.blas1_sum(fma, dt, ap, bp, LS.grid_for(len(ap), 8, nsm))
+                       for ap, bp in zip(rows(sizes, a), rows(sizes, b))]))
+
+
+def project(fma, sizes, Q, x, nsm):
+    """b2k_basis_project (and the projection of a classical pass): the fold of the ranks' per-pass colsums"""
+    return fold([ts.project(Qp, xp, nsm, fma) for Qp, xp in zip(rows(sizes, Q), rows(sizes, x))])
+
+
+def cgs_pass(fma, sizes, Q, v, nsm):
+    """one unfused classical pass (cgs_pass_unfused_t): (h, v', ||v'||^2)"""
+    dt = Q.dtype.type
+    h = project(fma, sizes, Q, v, nsm)
+    cs = ts.coefs(h, -1.0, dt)
+    out = [ts.update(Qp, vp, cs, fma) for Qp, vp in zip(rows(sizes, Q), rows(sizes, v))]
+    n2 = float(fold([ts.normsum(ts.norm_partials(w, nsm, fma)) for w in out]))
+    return h, np.concatenate(out), n2
+
+
+def mgs_sweep(fma, sizes, Q, v, nsm):
+    """mgs_sweep: each s_j folded before the next launch subtracts it.  (s, v')"""
+    dt = Q.dtype.type
+    xs = [np.asarray(x, dtype=dt) for x in rows(sizes, v)]
+    Qs = rows(sizes, Q)
+    s = []
+    for j in range(Q.shape[1]):
+        if j > 0:
+            xs = [fma(-dt(s[-1]), Qp[:, j - 1], x, dt) for Qp, x in zip(Qs, xs)]
+        s.append(float(fold([LS.blas1_sum(fma, dt, Qp[:, j], x, LS.grid_for(len(x), 8, nsm))
+                             for Qp, x in zip(Qs, xs)])))
+    xs = [fma(-dt(s[-1]), Qp[:, -1], x, dt) for Qp, x in zip(Qs, xs)]
+    return np.array(s), np.concatenate(xs)
+
+
+def orthogonalize(fma, sizes, Q, v, alg, eta, nsm):
+    """b2k_basis_orthogonalize on the shards: (h, ||v'||, passes, v')"""
+    dt = Q.dtype.type
+    CGS, MGS, CGS2, MGS2, CGSIR, MGSIR, MGS2B = range(7)
+
+    def one(v):
+        if alg in (CGS, CGS2, MGS2B, CGSIR):
+            return cgs_pass(fma, sizes, Q, v, nsm)
+        s, v = mgs_sweep(fma, sizes, Q, v, nsm)
+        return s, v, None
+
+    def norm2(v, n2):
+        return dot(fma, dt, sizes, v, v, nsm) if n2 is None else n2
+
+    if alg in (CGSIR, MGSIR):
+        nold = math.sqrt(dot(fma, dt, sizes, v, v, nsm))
+        h, passes = np.zeros(Q.shape[1]), 0
+        while True:
+            hp, v, n2 = one(v)
+            passes += 1
+            h = h + hp
+            nnew = math.sqrt(norm2(v, n2))
+            if not (EPS[dt] < nnew < eta * nold):
+                return h, nnew, passes, v
+            nold = nnew
+    passes = 2 if alg in (CGS2, MGS2, MGS2B) else 1
+    h, v, n2 = one(v)
+    if passes == 2:
+        h2, v, n2 = one(v)
+        h = h + h2
+    return h, math.sqrt(norm2(v, n2)), passes, v
+
+
+def vec_orthogonalize(fma, sizes, q, v, alg, eta, nsm):
+    """b2k_vec_orthogonalize on the shards (every s and ||v||^2 a k_dot, all-reduced): (s, ||v'||, v', passes)"""
+    dt = np.asarray(v).dtype.type
+    CGS, MGS, CGS2, MGS2, CGSIR, MGSIR, MGS2B = range(7)
+
+    def step(v):
+        s = dot(fma, dt, sizes, q, v, nsm)
+        return s, fma(-dt(s), q, v, dt)
+
+    if alg in (CGSIR, MGSIR):
+        nold = math.sqrt(dot(fma, dt, sizes, v, v, nsm))
+        s, v = step(v)
+        nnew = math.sqrt(dot(fma, dt, sizes, v, v, nsm))
+        passes = 1
+        while EPS[dt] < nnew < eta * nold:
+            nold = nnew
+            s1, v = step(v)
+            passes += 1
+            s += s1
+            nnew = math.sqrt(dot(fma, dt, sizes, v, v, nsm))
+        return s, nnew, v, passes
+    s, v = step(v)
+    passes = 1
+    if alg in (CGS2, MGS2, MGS2B):
+        s1, v = step(v)
+        passes = 2
+        s = s + s1
+    return s, math.sqrt(dot(fma, dt, sizes, v, v, nsm)), v, passes
+
+
+def lanczos_expand(fma, dt, sizes, V, r, beta_old, csr, spmv_kernel, spmv_grids, nsm, alg, eta=0.0):
+    """b2k_lanczos_expand on the shards for every orthogonalizer but CGS2 (lanczos_step): (w, v, alpha, beta,
+    passes), w and v global, passes = 1 + the reorthogonalisation passes of CGSIR / MGSIR (1 otherwise).  CGS /
+    CGSIR: the SpMV with the fused dot gives alpha0, the prologue is axpy2; CGSIR decides on beta = ||w'|| first and
+    then runs classical passes over [V, v] without a prologue.  The MGS family: w -= beta_old v_prev (axpby),
+    alpha0 = <v, w>, w -= alpha0 v, then nothing (MGS), one classical pass (MGS2B), one MGS sweep (MGS2) or the MGSIR
+    loop of sweeps; alpha += the coefficient of v.  MGS2B takes alpha0 from the SpMV epilogue (dotv = v, dot_sub_vec
+    = v_prev scaled by beta_old: the chained step's order), the others from k_dot after the SpMV."""
+    CGS, MGS, CGS2, MGS2, CGSIR, MGSIR, MGS2B = range(7)
+    off = offsets(sizes)
+    v = (dt(1.0 / beta_old) * np.asarray(r, dtype=dt)).astype(dt)
+    Q = np.column_stack([V, v])
+    classical = alg in (CGS, CGSIR)
+    fused = classical or alg == MGS2B
+    sub = dict(dsub=V[:, -1], dsc=beta_old) if alg == MGS2B else {}
+    ws, ds = [], []
+    for p, n in enumerate(sizes):
+        w, _, d = spmv(fma, dt, spmv_kernel, spmv_grids[p], v, off[p], n, csr=local_csr(*csr, off[p], n),
+                       dotv=v if fused else None, **sub)
+        ws.append(w)
+        ds.append(d)
+    w = np.concatenate(ws)
+    eps = EPS[dt]
+    passes = 1
+    if classical:
+        alpha = float(fold(ds))
+        w = ts.prologue(w, V[:, -1], v, beta_old, alpha, fma)
+        beta = math.sqrt(dot(fma, dt, sizes, w, w, nsm))
+        if alg == CGS:
+            return w, v, alpha, beta, passes
+        nold = math.sqrt(beta * beta + (alpha * alpha + beta_old * beta_old))
+        if not (eps < beta < eta * nold):
+            return w, v, alpha, beta, passes
+        nold = beta
+        while True:
+            h, w, n2 = cgs_pass(fma, sizes, Q, w, nsm)
+            passes += 1
+            alpha += float(h[-1])
+            beta = math.sqrt(n2)
+            if not (eps < beta < eta * nold):
+                return w, v, alpha, beta, passes
+            nold = beta
+    w = fma(-beta_old, V[:, -1], w, dt)
+    alpha = float(fold(ds)) if alg == MGS2B else dot(fma, dt, sizes, v, w, nsm)
+    w = fma(-dt(alpha), v, w, dt)
+    if alg == MGS2B:
+        h, w, n2 = cgs_pass(fma, sizes, Q, w, nsm)
+        return w, v, alpha + float(h[-1]), math.sqrt(n2), passes
+    if alg == MGS2:
+        s, w = mgs_sweep(fma, sizes, Q, w, nsm)
+        return w, v, alpha + float(s[-1]), math.sqrt(dot(fma, dt, sizes, w, w, nsm)), passes
+    beta = math.sqrt(dot(fma, dt, sizes, w, w, nsm))
+    if alg == MGSIR:
+        nold = math.sqrt(beta * beta + alpha * alpha + beta_old * beta_old)
+        while eps < beta < eta * nold:
+            nold = beta
+            s, w = mgs_sweep(fma, sizes, Q, w, nsm)
+            passes += 1
+            alpha += float(s[-1])
+            beta = math.sqrt(dot(fma, dt, sizes, w, w, nsm))
+    return w, v, alpha, beta, passes
+
+
+def sharded_apply(fma, dt, sizes, xg, csr, spmv_kernel, spmv_grids, dotv=None, **kw):
+    """the halo SpMV on every rank: (global y, the ranks' dot partials)"""
+    off = offsets(sizes)
+    ys, ds = [], []
+    for p, n in enumerate(sizes):
+        y, _, d = spmv(fma, dt, spmv_kernel, spmv_grids[p], xg, off[p], n, csr=local_csr(*csr, off[p], n),
+                       dotv=dotv, **kw)
+        ys.append(y)
+        ds.append(d)
+    return np.concatenate(ys), ds
+
+
+def shift_kw(a0, a1):
+    return dict(a0=a0, a1=a1, shifted=(a0 != 0.0) or (a1 != 1.0))
+
+
+def cg_step(fma, dt, sizes, x, r, p, csr, spmv_kernel, spmv_grids, nsm, a0, a1, beta, rho):
+    """b2k_cg_step on the shards: p' = r (beta = 0) or rn(r + rn(T(beta) p)); q' = (a0 + a1 A) p' with <p', q'>
+    fused (folded); alpha = T(rho / <p', q'>); x' = fma(alpha, p', x); r' = fma(-alpha, q', r); ||r'||^2 the fold of
+    k_cg_xr's sums.  (x', r', p', q', <p', q'>, ||r'||, the ranks' <p', q'> partials, the ranks' ||r'||^2 partials)"""
+    pn = np.asarray(r, dtype=dt).copy() if beta == 0.0 else (r + dt(beta) * p).astype(dt)
+    q, dpq = sharded_apply(fma, dt, sizes, pn, csr, spmv_kernel, spmv_grids, dotv=pn, **shift_kw(a0, a1))
+    pq = float(fold(dpq))
+    al = dt(rho / pq)
+    xn, rn = fma(al, pn, x, dt), fma(-al, q, r, dt)
+    drr = [LS.blas1_sum(fma, dt, a, a, LS.grid_for(len(a), 8, nsm)) for a in rows(sizes, rn)]
+    return xn, rn, pn, q, pq, math.sqrt(float(fold(drr))), dpq, drr
+
+
+def bicgstab_half(fma, dt, sizes, rs, r, p, v, csr, spmv_kernel, spmv_grids, nsm, a0, a1, beta, omega, rho, first):
+    """b2k_bicgstab_half on the shards: p' = r (first) or rn(r + rn(T(beta) fma(-T(omega), v, p))); v' = (a0 + a1 A)
+    p' with sigma = <rs, v'> fused (folded); s' = fma(-T(rho / sigma), v', r); ||s'||^2 the fold of k_bicg_s's sums.
+    (p', v', s', sigma, ||s'||, the sigma partials, the ||s'||^2 partials)"""
+    if first:
+        pn = np.asarray(r, dtype=dt).copy()
+    else:
+        pn = (r + dt(beta) * fma(-dt(omega), v, p, dt)).astype(dt)
+    vn, ds = sharded_apply(fma, dt, sizes, pn, csr, spmv_kernel, spmv_grids, dotv=rs, **shift_kw(a0, a1))
+    sigma = float(fold(ds))
+    sn = fma(-dt(rho / sigma), vn, r, dt)
+    dss = [LS.blas1_sum(fma, dt, a, a, LS.grid_for(len(a), 8, nsm)) for a in rows(sizes, sn)]
+    return pn, vn, sn, sigma, math.sqrt(float(fold(dss))), ds, dss
+
+
+def bicgstab_full(fma, dt, sizes, x, rs, p, s, csr, spmv_kernel, spmv_grids, nsm, a0, a1, alpha):
+    """b2k_bicgstab_full on the shards: t' = (a0 + a1 A) s with <t', s> fused, <t', t'> by k_dot (both folded, one
+    all-reduce of two doubles); omega = <t', s> / <t', t'>; x' = fma(T(omega), s, fma(T(alpha), p, x));
+    r' = fma(-T(omega), t', s); ||r'||^2 and <rs, r'> the folds of k_bicg_xr's sums.
+    (x', r', t', omega, ||r'||, next rho, the partials of <t', s>, <t', t'>, ||r'||^2 and <rs, r'>)"""
+    tn, dts = sharded_apply(fma, dt, sizes, s, csr, spmv_kernel, spmv_grids, dotv=s, **shift_kw(a0, a1))
+    dtt = [LS.blas1_sum(fma, dt, a, a, LS.grid_for(len(a), 8, nsm)) for a in rows(sizes, tn)]
+    omega = float(fold(dts)) / float(fold(dtt))
+    w = dt(omega)
+    xn = fma(w, s, fma(dt(alpha), p, x, dt), dt)
+    rn = fma(-w, tn, s, dt)
+    drr = [LS.blas1_sum(fma, dt, a, a, LS.grid_for(len(a), 8, nsm)) for a in rows(sizes, rn)]
+    drho = [LS.blas1_sum(fma, dt, a, b, LS.grid_for(len(a), 8, nsm)) for a, b in zip(rows(sizes, rs), rows(sizes, rn))]
+    return xn, rn, tn, omega, math.sqrt(float(fold(drr))), float(fold(drho)), (dts, dtt, drr, drho)
+
+
+def dense_adjoint(fma, sizes, A, x, nsm):
+    """b2k_op_apply_adjoint of a row-sharded dense A (m x n): y = T(fold of the ranks' per-pass project colsums of
+    their row blocks against x_p), the same on every rank"""
+    dt = A.dtype.type
+    return project(fma, sizes, A, x, nsm).astype(dt)

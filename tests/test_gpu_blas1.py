@@ -39,6 +39,8 @@ from krylovkit_jl_b200 import _lib as L
 from krylovkit_jl_b200.vectors import handles
 from oracle import krylov_oracle as ko
 from test_gpu_paths import LAM, SPMV, profiled, unit
+import lsmr_restate as LS
+import spmv_restate as SR
 
 SEED = 20260923
 f64, f32 = np.float64, np.float32
@@ -453,6 +455,22 @@ def cg_step(ctx, op, vs, a0, a1, beta, rho):
     return pq.value, nr.value
 
 
+def fused_dot(fma, dt, op, x, dotv, a0, a1):
+    """the dot the last SpMV launch fused into its epilogue, in spmv_restate's order on the grid it reported"""
+    from test_gpu_spmv_fused import launch
+    kid, _, grid, _ = launch()
+    A = op.to_scipy()
+    csr = (A.indptr, A.indices, A.data.astype(dt))
+    kname = {1: "stream", 2: "pipe", 3: "compact"}[kid]
+    return SR.apply(fma, dt, kname, grid, x, csr=csr, rowblk=SR.tiles(A.indptr), a0=a0, a1=a1,
+                    shifted=(a0 != 0.0) or (a1 != 1.0), dotv=dotv)[2]
+
+
+def stream_sum(fma, dt, a, b):
+    """a k_dot / k_cg_xr / k_bicg_s / k_bicg_xr sum: lsmr_restate.blas1_sum on grid_for(n, 8)"""
+    return LS.blas1_sum(fma, dt, a, b, grid_for(len(a)))
+
+
 def dot_bound(dt, a, b):
     """|computed - exact| of an n-term sum of products in T"""
     return LAM * math.sqrt(a.size) * unit(dt) * float(np.abs(a.astype(f64) * b.astype(f64)).sum())
@@ -475,6 +493,7 @@ def test_cg_step_bitwise(dt, beta, shift, fma):
     pq, nr = cg_step(ctx, op, (x, r, p, q), a0, a1, beta, rho)
     pn = rh if beta == 0.0 else rh + dt(beta) * ph
     assert np.array_equal(p.to_host(), pn)
+    assert pq == fused_dot(fma, dt, op, pn, pn, a0, a1)
     qn = kk.apply(op, ctx.from_host(pn), a0, a1).to_host()
     assert np.array_equal(q.to_host(), qn)
     assert abs(pq - math.fsum(pn.astype(f64) * qn.astype(f64))) <= dot_bound(dt, pn, qn)
@@ -483,6 +502,7 @@ def test_cg_step_bitwise(dt, beta, shift, fma):
     rn = fma(-al, qn, rh, dt)
     assert np.array_equal(r.to_host(), rn)
     assert abs(nr ** 2 - math.fsum(rn.astype(f64) ** 2)) <= 2 * dot_bound(dt, rn, rn)
+    assert nr == math.sqrt(stream_sum(fma, dt, rn, rn))
     ctx.close()
 
 
@@ -618,6 +638,7 @@ def test_bicgstab_half_and_full_bitwise(dt, shift, first, fma):
     sigma, ns = bicg_half(ctx, op, rs, r, p, v, s, a0, a1, beta, omega, rho, first)
     pn = rh if first else rh + dt(beta) * fma(-dt(omega), vh, ph, dt)
     assert np.array_equal(p.to_host(), pn)
+    assert sigma == fused_dot(fma, dt, op, pn, rsh, a0, a1)
     vn = kk.apply(op, ctx.from_host(pn), a0, a1).to_host()
     assert np.array_equal(v.to_host(), vn)
     assert abs(sigma - math.fsum(rsh.astype(f64) * vn.astype(f64))) <= dot_bound(dt, rsh, vn)
@@ -625,7 +646,9 @@ def test_bicgstab_half_and_full_bitwise(dt, shift, first, fma):
     sn = fma(-dt(alpha), vn, rh, dt)
     assert np.array_equal(s.to_host(), sn)
     assert abs(ns ** 2 - math.fsum(sn.astype(f64) ** 2)) <= 2 * dot_bound(dt, sn, sn)
+    assert ns == math.sqrt(stream_sum(fma, dt, sn, sn))
     om, nr, rho_next = bicg_full(ctx, op, x, r, rs, p, s, t, a0, a1, alpha)
+    ts_exact = fused_dot(fma, dt, op, sn, sn, a0, a1)
     tn = kk.apply(op, ctx.from_host(sn), a0, a1).to_host()
     assert np.array_equal(t.to_host(), tn)
     ts, tt = math.fsum(tn.astype(f64) * sn.astype(f64)), math.fsum(tn.astype(f64) ** 2)
@@ -637,6 +660,8 @@ def test_bicgstab_half_and_full_bitwise(dt, shift, first, fma):
     assert np.array_equal(r.to_host(), rn)
     assert abs(nr ** 2 - math.fsum(rn.astype(f64) ** 2)) <= 2 * dot_bound(dt, rn, rn)
     assert abs(rho_next - math.fsum(rsh.astype(f64) * rn.astype(f64))) <= dot_bound(dt, rsh, rn)
+    assert om == ts_exact / stream_sum(fma, dt, tn, tn)
+    assert nr == math.sqrt(stream_sum(fma, dt, rn, rn)) and rho_next == stream_sum(fma, dt, rsh, rn)
     # the literal sequence (USE_FUSED_BICGSTAB = False) with the same scalars, vector for vector
     r, x = ctx.from_host(rh), ctx.from_host(xh)
     if first:

@@ -1,5 +1,6 @@
 """The row-sharded path bit for bit (tests/dist_restate_worker.py under torchrun): the halo SpMV kernels with every
-fused feature, the rank-ordered sums and the sharded Lanczos step against the composed restatement of
+fused feature, the rank-ordered sums, the sharded Lanczos step with every orthogonalizer, project / orthogonalize, the
+CG and BiCGStab steps, the block path, the dense adjoint and a replicated space against the composed restatement of
 tests/dist_restate.py.  Two and three ranks always share GPU 0 (peer window only, gloo for the worker's gathers); with
 at least 2 GPUs the job also runs with one rank per GPU, on the peer window and on NCCL (B2K_PEER=0).
 
