@@ -1351,10 +1351,14 @@ int32_t cgs_pass_unfused_t(b2k_ctx* ctx, const Panel& pn, const VecRef& v, int k
     return B2K_OK;
 }
 
-bool fused_ok(const b2k_ctx* ctx, int k, int sharded, int dtype) {
+// whether ncols columns fit the panel ring of the cooperative sweep (C columns per chunk)
+bool ring_holds(int dtype, int ncols) {
     const int C = dtype == B2K_F64 ? 8 : 16;
-    const int nch = (k + C - 1) / C;
-    return !(ctx->nranks > 1 && sharded) && nch <= NS && k <= MAXCH * C;
+    return (ncols + C - 1) / C <= NS && ncols <= MAXCH * C;
+}
+
+bool fused_ok(const b2k_ctx* ctx, int k, int sharded, int dtype) {
+    return !(ctx->nranks > 1 && sharded) && ring_holds(dtype, k);
 }
 
 bool g_use_coop = true;
@@ -1522,8 +1526,7 @@ extern "C" int32_t b2k_basis_project(b2k_ctx* ctx, const b2k_vec* cols, int32_t 
     B2K_TRY(b2k_resolve(ctx, x, &rx));
     if (rx.n != pn.n) return b2k_fail(ctx, B2K_EDIM, "basis_project: x has %lld rows, basis %lld",
                                       (long long)rx.n, (long long)pn.n);
-    if (ctx->dtype == B2K_F64) B2K_TRY(project_t<double>(ctx, pn, rx, k, 0));
-    else B2K_TRY(project_t<float>(ctx, pn, rx, k, 0));
+    B2K_TRY(b2k_dispatch(ctx, [&](auto t) { return project_t<decltype(t)>(ctx, pn, rx, k, 0); }));
     B2K_TRY(b2k_fetch_results(ctx, k, pn.sharded));
     for (int j = 0; j < k; ++j)
         h_host[j] = (beta == 0.0) ? alpha * ctx->h_res[j] : beta * h_host[j] + alpha * ctx->h_res[j];
@@ -1548,9 +1551,9 @@ extern "C" int32_t b2k_basis_unproject(b2k_ctx* ctx, b2k_vec y, const b2k_vec* c
         if (pn.idx[j] == ry.col && ry.space == B2K_VEC_SPACE(cols[j]))
             return b2k_fail(ctx, B2K_EINVAL, "basis_unproject: y aliases basis vector %d", j);
     B2K_TRY(b2k_put_coef(ctx, c_host, k, 0));
-    if (ctx->dtype == B2K_F64)
-        return unproject_t<double>(ctx, pn, ry, k, ctx->d_coef, nullptr, alpha, beta, nullptr);
-    return unproject_t<float>(ctx, pn, ry, k, ctx->d_coef, nullptr, alpha, beta, nullptr);
+    return b2k_dispatch(ctx, [&](auto t) {
+        return unproject_t<decltype(t)>(ctx, pn, ry, k, ctx->d_coef, nullptr, alpha, beta, nullptr);
+    });
 }
 
 // internal: used by the dense operator (spmv.cu): y = A x / y = A' x through the engine
@@ -1560,9 +1563,10 @@ int32_t b2k_panel_unproject_dev(b2k_ctx* ctx, void* base, int64_t ld, int64_t n,
     pn.base = base; pn.ld = ld; pn.n = n; pn.sharded = y.sharded;
     pn.idx.resize(k);
     for (int i = 0; i < k; ++i) pn.idx[i] = i;
-    if (ctx->dtype == B2K_F64)
-        return unproject_t<double>(ctx, pn, y, k, nullptr, (const double*)coef_t, 1.0, 0.0, nullptr);
-    return unproject_t<float>(ctx, pn, y, k, nullptr, (const float*)coef_t, 1.0, 0.0, nullptr);
+    return b2k_dispatch(ctx, [&](auto t) {
+        using T = decltype(t);
+        return unproject_t<T>(ctx, pn, y, k, nullptr, (const T*)coef_t, 1.0, 0.0, nullptr);
+    });
 }
 
 int32_t b2k_panel_project_dev(b2k_ctx* ctx, void* base, int64_t ld, int64_t n, int32_t k,
@@ -1572,14 +1576,13 @@ int32_t b2k_panel_project_dev(b2k_ctx* ctx, void* base, int64_t ld, int64_t n, i
     pn.idx.resize(k);
     for (int i = 0; i < k; ++i) pn.idx[i] = i;
     if (k > B2K_RES_DOUBLES) return b2k_fail(ctx, B2K_ENOTSUP, "dense adjoint: too many columns");
-    if (ctx->dtype == B2K_F64) B2K_TRY(project_t<double>(ctx, pn, x, k, 0));
-    else B2K_TRY(project_t<float>(ctx, pn, x, k, 0));
+    B2K_TRY(b2k_dispatch(ctx, [&](auto t) { return project_t<decltype(t)>(ctx, pn, x, k, 0); }));
     B2K_TRY(b2k_allreduce(ctx, ctx->d_res, k, sharded));
     const int blocks = (k + 127) / 128;
-    if (ctx->dtype == B2K_F64)
-        k_res_to_vec<double><<<blocks, 128, 0, ctx->stream>>>(ctx->d_res, (double*)out_vec, k, 1.0);
-    else
-        k_res_to_vec<float><<<blocks, 128, 0, ctx->stream>>>(ctx->d_res, (float*)out_vec, k, 1.0f);
+    b2k_dispatch(ctx, [&](auto t) {
+        using T = decltype(t);
+        k_res_to_vec<T><<<blocks, 128, 0, ctx->stream>>>(ctx->d_res, (T*)out_vec, k, T(1));
+    });
     B2K_LAUNCH_CHECK(ctx);
     return B2K_OK;
 }
@@ -1605,21 +1608,18 @@ extern "C" int32_t b2k_basis_orthogonalize(b2k_ctx* ctx, b2k_vec v, const b2k_ve
     for (int j = 0; j < k; ++j)
         if (pn.idx[j] == rv.col && rv.space == B2K_VEC_SPACE(cols[j]))
             return b2k_fail(ctx, B2K_EINVAL, "basis_orthogonalize: v aliases basis vector %d", j);
-    const bool f64 = ctx->dtype == B2K_F64;
     const bool fusable = fused_ok(ctx, k, pn.sharded, ctx->dtype);
-    const double eps = f64 ? 0x1p-52 : 0x1p-23;   // eps(T) of the IR loops (orthonormal.jl, lanczos.jl)
+    const double eps = b2k_eps(ctx);   // of the IR loops (orthonormal.jl, lanczos.jl)
     const int NS_ = 2 * k + 4;   // slot of ||v||^2 results for unfused / MGS paths
 
     auto cgs_passes = [&](int passes) -> int32_t {   // leaves h in h_res[0..k), norm^2 in h_res[k]
         if (fusable) {
-            if (f64) B2K_TRY(cgs_fused_t<double>(ctx, pn, rv, k, passes, g_use_coop));
-            else B2K_TRY(cgs_fused_t<float>(ctx, pn, rv, k, passes, g_use_coop));
+            B2K_TRY(b2k_dispatch(ctx, [&](auto t) { return cgs_fused_t<decltype(t)>(ctx, pn, rv, k, passes, g_use_coop); }));
             return b2k_fetch_results(ctx, k + 1, 0);
         }
         // unfused: pass p writes h_p to d_res[p*k ..], norm to d_res[NS_]
         for (int ps = 0; ps < passes; ++ps) {
-            if (f64) B2K_TRY(cgs_pass_unfused_t<double>(ctx, pn, rv, k, ps * k, NS_));
-            else B2K_TRY(cgs_pass_unfused_t<float>(ctx, pn, rv, k, ps * k, NS_));
+            B2K_TRY(b2k_dispatch(ctx, [&](auto t) { return cgs_pass_unfused_t<decltype(t)>(ctx, pn, rv, k, ps * k, NS_); }));
         }
         B2K_TRY(b2k_fetch_results(ctx, NS_ + 1, 0));
         if (passes == 2)
@@ -1700,9 +1700,8 @@ extern "C" int32_t b2k_lanczos_expand(b2k_ctx* ctx, const b2k_op* op, const b2k_
     if (rv.n != pn.n || rw.n != pn.n) return b2k_fail(ctx, B2K_EDIM, "lanczos_expand: length mismatch");
     for (int j = 0; j <= k; ++j)
         if (cols[j] == w) return b2k_fail(ctx, B2K_EINVAL, "lanczos_expand: w aliases the basis");
-    const bool f64 = ctx->dtype == B2K_F64;
     const int K1 = k + 1;
-    const double eps = f64 ? 0x1p-52 : 0x1p-23;   // eps(T) of the IR loops (orthonormal.jl, lanczos.jl)
+    const double eps = b2k_eps(ctx);   // of the IR loops (orthonormal.jl, lanczos.jl)
     // d_res slots
     const int S_H = 0;             // [0..K1) projection coefficients
     const int S_N = K1;            // ||w||^2
@@ -1717,7 +1716,7 @@ extern "C" int32_t b2k_lanczos_expand(b2k_ctx* ctx, const b2k_op* op, const b2k_
         B2K_TRY(b2k_allreduce(ctx, ctx->d_res + S_A0, 1, pn.sharded));
         // CGS2 on the fused path keeps alpha on the device (the prologue reads it from d_res) so
         // that the whole step needs ONE host synchronisation; the other variants fetch it now.
-        const bool one_pass = K1 <= (f64 ? kcap<double>() : kcap<float>());
+        const bool one_pass = K1 <= b2k_dispatch(ctx, [](auto t) { return kcap<decltype(t)>(); });
         const bool defer_alpha = (alg == B2K_CGS2) && one_pass;
         double alpha = 0.0;
         if (!defer_alpha) {
@@ -1756,18 +1755,15 @@ extern "C" int32_t b2k_lanczos_expand(b2k_ctx* ctx, const b2k_op* op, const b2k_
             }
             if (one_pass) {
                 const double* c2_dev = defer_alpha ? ctx->d_res + S_A0 : nullptr;
-                if (f64)
-                    B2K_TRY(lanczos_step_gs<double>(ctx, pn, K1, rw, prologue, -beta_old, -alpha, c2_dev, fusable,
-                                                    S_H, S_N));
-                else
-                    B2K_TRY(lanczos_step_gs<float>(ctx, pn, K1, rw, prologue, -beta_old, -alpha, c2_dev, fusable,
-                                                   S_H, S_N));
+                B2K_TRY(b2k_dispatch(ctx, [&](auto t) {
+                    return lanczos_step_gs<decltype(t)>(ctx, pn, K1, rw, prologue, -beta_old, -alpha, c2_dev, fusable,
+                                                        S_H, S_N);
+                }));
                 B2K_TRY(b2k_fetch_results(ctx, S_A0 + 1, 0));
                 if (defer_alpha) alpha = ctx->h_res[S_A0];
             } else {
                 if (prologue) B2K_TRY(b2k_vec_axpy2(ctx, w, cols[k - 1], -beta_old, r, -alpha));
-                if (f64) B2K_TRY(cgs_pass_unfused_t<double>(ctx, pn, rw, K1, S_H, S_N));
-                else B2K_TRY(cgs_pass_unfused_t<float>(ctx, pn, rw, K1, S_H, S_N));
+                B2K_TRY(b2k_dispatch(ctx, [&](auto t) { return cgs_pass_unfused_t<decltype(t)>(ctx, pn, rw, K1, S_H, S_N); }));
                 B2K_TRY(b2k_fetch_results(ctx, S_N + 1, 0));
             }
             alpha += ctx->h_res[S_H + k];        // α += s[end]
@@ -1813,11 +1809,9 @@ extern "C" int32_t b2k_lanczos_expand(b2k_ctx* ctx, const b2k_op* op, const b2k_
     } else if (alg == B2K_MGS2B) {
         // flagged: the second sweep over all of V as ONE classical pass (project, update + norm)
         if (fused_ok(ctx, K1, pn.sharded, ctx->dtype)) {
-            if (f64) B2K_TRY(cgs_fused_t<double>(ctx, pn, rw, K1, 1, g_use_coop));
-            else B2K_TRY(cgs_fused_t<float>(ctx, pn, rw, K1, 1, g_use_coop));
+            B2K_TRY(b2k_dispatch(ctx, [&](auto t) { return cgs_fused_t<decltype(t)>(ctx, pn, rw, K1, 1, g_use_coop); }));
         } else {
-            if (f64) B2K_TRY(cgs_pass_unfused_t<double>(ctx, pn, rw, K1, S_H, S_N));
-            else B2K_TRY(cgs_pass_unfused_t<float>(ctx, pn, rw, K1, S_H, S_N));
+            B2K_TRY(b2k_dispatch(ctx, [&](auto t) { return cgs_pass_unfused_t<decltype(t)>(ctx, pn, rw, K1, S_H, S_N); }));
         }
         B2K_TRY(b2k_fetch_results(ctx, S_A0 + 1, 0));
         alpha = ctx->h_res[S_A0] + ctx->h_res[S_H + k];   // α += s (coefficient vs V[end])
@@ -1888,9 +1882,8 @@ bool chain_ok(const b2k_ctx* ctx, const b2k_op* op, const b2k_vec* cols, int32_t
     } else if (op_rows != s.n || op_cols != s.n) {
         return false;
     }
-    const int C = ctx->dtype == B2K_F64 ? 8 : 16;
     const int K1 = k + nsteps;
-    return (K1 + C - 1) / C <= NS && K1 <= MAXCH * C && K1 <= PEER_SLOT;
+    return ring_holds(ctx->dtype, K1) && K1 <= PEER_SLOT;
 }
 
 // The cooperative CGS sweep of one chained step over the K1 columns of pn, finalised into the device record rec.
@@ -1956,18 +1949,16 @@ int32_t chain_step_gs(b2k_ctx* ctx, const Panel& pn, int K1, const VecRef& rw, d
 int32_t lanczos_chain(b2k_ctx* ctx, const b2k_op* op, b2k_vec* cols, int32_t k, int32_t nsteps,
                       double beta_old, double tol, int32_t alg, double* alphas_out, double* betas_out,
                       int32_t* steps_done, b2k_vec* r_out) {
-    const bool f64 = ctx->dtype == B2K_F64;
     const int32_t space = B2K_VEC_SPACE(cols[k]);
-    double* rec0 = ctx->d_steps;
-    int* d_stop = reinterpret_cast<int*>(ctx->d_sync + B2K_SYNC_STOP);
     {   // every handle must be live before anything is enqueued
         VecRef t;
         for (int i = 0; i <= k; ++i) B2K_TRY(b2k_resolve(ctx, cols[i], &t));
     }
-    k_lanczos_seed<<<1, 1, 0, ctx->stream>>>(rec0, beta_old, d_stop);
+    // record i of the batch is rec_{i-1} of the step protocol below; the seed is rec_{-1}
+    B2kChain fr(ctx, B2K_REC);
+    k_lanczos_seed<<<1, 1, 0, ctx->stream>>>(fr.st, beta_old, fr.stop);
     B2K_LAUNCH_CHECK(ctx);
-    std::vector<b2k_vec> touched, Vh, Wh;
-    touched.push_back(cols[k]);
+    B2kChainCols cc(ctx, cols[k]);
     int32_t enq = 0, rc = B2K_OK;
     const bool dist = ctx->nranks > 1;
     unsigned long long halo_seq = 0;
@@ -1975,25 +1966,20 @@ int32_t lanczos_chain(b2k_ctx* ctx, const b2k_op* op, b2k_vec* cols, int32_t k, 
         const int32_t K = k + i;                 // basis size before this step's push!
         const b2k_vec R = cols[K];
         b2k_vec V = -1, W = -1;
-        rc = b2k_vec_alloc(ctx, space, &V);
-        if (rc != B2K_OK) break;
-        touched.push_back(V);
-        rc = b2k_vec_alloc(ctx, space, &W);
-        if (rc != B2K_OK) break;
-        touched.push_back(W);
+        if ((rc = cc.alloc(space, &V)) != B2K_OK || (rc = cc.alloc(space, &W)) != B2K_OK) break;
         VecRef rR, rV, rW, vprev;
         rc = b2k_resolve(ctx, R, &rR);
         if (rc == B2K_OK) rc = b2k_resolve(ctx, V, &rV);
         if (rc == B2K_OK) rc = b2k_resolve(ctx, W, &rW);
         if (rc == B2K_OK) rc = b2k_resolve(ctx, cols[K - 1], &vprev);
         if (rc != B2K_OK) break;
-        double* rec_prev = rec0 + (size_t)B2K_REC * i;
-        double* rec = rec0 + (size_t)B2K_REC * (i + 1);
+        double* rec_prev = fr.st + (size_t)B2K_REC * i;
+        double* rec = fr.rec0 + (size_t)B2K_REC * i;
         SpmvFuse fz;
         memset(&fz, 0, sizeof(fz));
         fz.xscale = rec_prev + 3;
         fz.vout = rV.ptr;
-        fz.stop = d_stop;
+        fz.stop = fr.stop;
         fz.dot_self = 1;
         fz.l2_hints = g_l2_hints ? 1 : 0;
         fz.trace = ctx->d_trace;
@@ -2021,46 +2007,28 @@ int32_t lanczos_chain(b2k_ctx* ctx, const b2k_op* op, b2k_vec* cols, int32_t k, 
         Panel pn;
         rc = make_panel(ctx, cols, K + 1, &pn);
         if (rc != B2K_OK) break;
-        rc = f64 ? chain_step_gs<double>(ctx, pn, K + 1, rW, rec_prev, rec, tol, &ps)
-                 : chain_step_gs<float>(ctx, pn, K + 1, rW, rec_prev, rec, tol, &ps);
+        rc = b2k_dispatch(ctx, [&](auto t) {
+            return chain_step_gs<decltype(t)>(ctx, pn, K + 1, rW, rec_prev, rec, tol, &ps);
+        });
         if (rc != B2K_OK) break;
         cols[K + 1] = W;                         // ... and w the new residual
-        Vh.push_back(V);
-        Wh.push_back(W);
-        // r's column has been consumed; later steps may reuse it (stream order keeps that safe)
-        ctx->spaces[space].used[B2K_VEC_COL(R)] = 0;
+        cc.ran(V, -1, W);
+        cc.consumed(R);
         ++enq;
     }
     int32_t d = 0;
     if (enq > 0) {
-        cudaError_t e = cudaMemcpyAsync(ctx->h_res, rec0 + B2K_REC, sizeof(double) * B2K_REC * enq,
-                                        cudaMemcpyDeviceToHost, ctx->stream);
-        if (e != cudaSuccess)
-            return b2k_fail(ctx, B2K_ECUDA, "lanczos_expand_many: %s", cudaGetErrorString(e));
-        B2K_TRY(b2k_stream_sync(ctx));           // ... and the peer-window watchdog latch of the batch
-        d = enq;
-        for (int32_t i = 0; i < enq; ++i) {
-            alphas_out[i] = ctx->h_res[(size_t)B2K_REC * i + 1];
-            betas_out[i] = ctx->h_res[(size_t)B2K_REC * i + 2];
-            if (betas_out[i] <= tol) { d = i + 1; break; }
+        B2K_TRY(fr.fetch(enq));                  // ... and the peer-window watchdog latch of the batch
+        d = fr.count(enq, [&](const double* r) { return r[2] <= tol; });
+        for (int32_t i = 0; i < d; ++i) {
+            alphas_out[i] = fr.hrec[(size_t)B2K_REC * i + 1];
+            betas_out[i] = fr.hrec[(size_t)B2K_REC * i + 2];
         }
     } else {
-        cudaStreamSynchronize(ctx->stream);
-    }
-    // column bookkeeping: everything this batch touched is free again, except the d new basis vectors and
-    // the residual that follows them (steps behind a breakdown were skipped on the device)
-    B2kSpace& sp = ctx->spaces[space];
-    for (b2k_vec h : touched) sp.used[B2K_VEC_COL(h)] = 0;
-    if (d > 0) {
-        for (int32_t i = 0; i < d; ++i) cols[k + i] = Vh[i];     // (skipped steps overwrote cols[k + d ..])
-        cols[k + d] = Wh[d - 1];
-        for (int32_t i = 0; i <= d; ++i) sp.used[B2K_VEC_COL(cols[k + i])] = 1;
-    } else {
-        sp.used[B2K_VEC_COL(touched[0])] = 1;    // nothing ran: r is still r
-        cols[k] = touched[0];
+        fr.fail(rc);
     }
     *steps_done = d;
-    *r_out = cols[k + d];
+    *r_out = cc.commit(d, cols, nullptr, k);
     return rc;
 }
 
@@ -2152,9 +2120,8 @@ int32_t gkl_refuse(b2k_ctx* ctx, const b2k_op* A, const b2k_op* At, const b2k_ve
             return b2k_fail(ctx, B2K_EDIM, "gkl_expand_many: V must be columns of one space of length %lld",
                             (long long)n);
     }
-    const int C = ctx->dtype == B2K_F64 ? 8 : 16;
     const int K1 = k + nsteps;
-    if ((K1 + C - 1) / C > NS || K1 > MAXCH * C || K1 > 256)
+    if (!ring_holds(ctx->dtype, K1) || K1 > 256)
         return b2k_fail(ctx, B2K_ENOTSUP, "gkl_expand_many: %d columns do not fit the sweep's panel ring", K1);
     return B2K_OK;
 }
@@ -2162,21 +2129,18 @@ int32_t gkl_refuse(b2k_ctx* ctx, const b2k_op* A, const b2k_op* At, const b2k_ve
 int32_t gkl_chain(b2k_ctx* ctx, const b2k_op* A, const b2k_op* At, b2k_vec* ucols, b2k_vec* vcols, int32_t k,
                   int32_t nsteps, double beta_old, double tol, int32_t alg, double* alphas_out, double* betas_out,
                   int32_t* steps_done, b2k_vec* r_out) {
-    const bool f64 = ctx->dtype == B2K_F64;
     const int32_t su = B2K_VEC_SPACE(ucols[k]), sv = B2K_VEC_SPACE(vcols[0]);
-    double* rec0 = ctx->d_steps;
-    int* d_stop = reinterpret_cast<int*>(ctx->d_sync + B2K_SYNC_STOP);
-    k_lanczos_seed<<<1, 1, 0, ctx->stream>>>(rec0, beta_old, d_stop);
+    B2kChain fr(ctx, B2K_REC);                   // record i of the batch is rec_{i-1} below; the seed is rec_{-1}
+    k_lanczos_seed<<<1, 1, 0, ctx->stream>>>(fr.st, beta_old, fr.stop);
     B2K_LAUNCH_CHECK(ctx);
-    std::vector<b2k_vec> touched, Uh, Vh, Wh;
-    touched.push_back(ucols[k]);
+    B2kChainCols cc(ctx, ucols[k]);
     GklFlush fl;
     memset(&fl, 0, sizeof(fl));
     int32_t enq = 0, rc = B2K_OK;
     auto fuse = [&]() {
         SpmvFuse fz;
         memset(&fz, 0, sizeof(fz));
-        fz.stop = d_stop;
+        fz.stop = fr.stop;
         fz.l2_hints = g_l2_hints ? 1 : 0;
         fz.trace = ctx->d_trace;
         return fz;
@@ -2185,12 +2149,8 @@ int32_t gkl_chain(b2k_ctx* ctx, const b2k_op* A, const b2k_op* At, b2k_vec* ucol
         const int32_t K = k + i;                 // basis size before this step
         const b2k_vec R = ucols[K];
         b2k_vec Vc = -1, Uc = -1, W = -1;
-        if ((rc = b2k_vec_alloc(ctx, sv, &Vc)) != B2K_OK) break;
-        touched.push_back(Vc);
-        if ((rc = b2k_vec_alloc(ctx, su, &Uc)) != B2K_OK) break;
-        touched.push_back(Uc);
-        if ((rc = b2k_vec_alloc(ctx, su, &W)) != B2K_OK) break;
-        touched.push_back(W);
+        if ((rc = cc.alloc(sv, &Vc)) != B2K_OK || (rc = cc.alloc(su, &Uc)) != B2K_OK || (rc = cc.alloc(su, &W)) != B2K_OK)
+            break;
         VecRef rR, rV, rU, rW, vprev;
         rc = b2k_resolve(ctx, R, &rR);
         if (rc == B2K_OK) rc = b2k_resolve(ctx, Vc, &rV);
@@ -2198,8 +2158,8 @@ int32_t gkl_chain(b2k_ctx* ctx, const b2k_op* A, const b2k_op* At, b2k_vec* ucol
         if (rc == B2K_OK) rc = b2k_resolve(ctx, W, &rW);
         if (rc == B2K_OK) rc = b2k_resolve(ctx, vcols[K - 1], &vprev);
         if (rc != B2K_OK) break;
-        double* rec_prev = rec0 + (size_t)B2K_REC * i;
-        double* rec = rec0 + (size_t)B2K_REC * (i + 1);
+        double* rec_prev = fr.st + (size_t)B2K_REC * i;
+        double* rec = fr.rec0 + (size_t)B2K_REC * i;
         // 1. v~_k = A' (r / beta) - beta v_{k-1}, finishing v_{k-1} on the way (the caller's V[k-1] is final)
         SpmvFuse fa = fuse();
         fa.xscale = rec_prev + 3;
@@ -2215,8 +2175,9 @@ int32_t gkl_chain(b2k_ctx* ctx, const b2k_op* A, const b2k_op* At, b2k_vec* ucol
         if (alg == B2K_MGS2B) {                  // the flagged MGS2B: v~_k -= V V' v~_k, alpha from the finaliser
             Panel pv;
             if ((rc = make_panel(ctx, vcols, K, &pv)) != B2K_OK) break;
-            rc = f64 ? chain_step_gs<double>(ctx, pv, K, rV, nullptr, rec + 3, -INFINITY, nullptr, false, 1)
-                     : chain_step_gs<float>(ctx, pv, K, rV, nullptr, rec + 3, -INFINITY, nullptr, false, 1);
+            rc = b2k_dispatch(ctx, [&](auto t) {
+                return chain_step_gs<decltype(t)>(ctx, pv, K, rV, nullptr, rec + 3, -INFINITY, nullptr, false, 1);
+            });
             if (rc != B2K_OK) break;
         }
         // 2. r' = A (v~_k / alpha) - alpha u_k, u_k = r / beta stored to its column
@@ -2231,60 +2192,41 @@ int32_t gkl_chain(b2k_ctx* ctx, const b2k_op* A, const b2k_op* At, b2k_vec* ucol
         // 3. r' -= U U' r', beta = ||r'||
         Panel pu;
         if ((rc = make_panel(ctx, ucols, K + 1, &pu)) != B2K_OK) break;
-        rc = f64 ? chain_step_gs<double>(ctx, pu, K + 1, rW, rec_prev, rec, tol, nullptr, false, 1)
-                 : chain_step_gs<float>(ctx, pu, K + 1, rW, rec_prev, rec, tol, nullptr, false, 1);
+        rc = b2k_dispatch(ctx, [&](auto t) {
+            return chain_step_gs<decltype(t)>(ctx, pu, K + 1, rW, rec_prev, rec, tol, nullptr, false, 1);
+        });
         if (rc != B2K_OK) break;
         ucols[K + 1] = W;
-        Uh.push_back(Uc);
-        Vh.push_back(Vc);
-        Wh.push_back(W);
+        cc.ran(Uc, Vc, W);
         fl.col[i] = B2K_VEC_COL(Vc);
-        // r's column has been read for the last time; later steps may reuse it (stream order keeps that safe)
-        ctx->spaces[su].used[B2K_VEC_COL(R)] = 0;
+        cc.consumed(R);
         ++enq;
-    }
-    if (enq > 0) {
-        const B2kSpace& s = ctx->spaces[sv];
-        fl.rec0 = rec0; fl.tol = tol; fl.nsteps = enq; fl.ld = s.ld; fl.n = s.n;
-        const int grid = (int)std::max<int64_t>(1, std::min<int64_t>((s.n + 255) / 256, (int64_t)ctx->num_sms * 4));
-        if (f64) k_gkl_flush<double><<<grid, 256, 0, ctx->stream>>>((double*)s.base, fl);
-        else k_gkl_flush<float><<<grid, 256, 0, ctx->stream>>>((float*)s.base, fl);
-        B2K_LAUNCH_CHECK(ctx);
     }
     int32_t d = 0;
     if (enq > 0) {
-        cudaError_t e = cudaMemcpyAsync(ctx->h_res, rec0 + B2K_REC, sizeof(double) * B2K_REC * enq,
-                                        cudaMemcpyDeviceToHost, ctx->stream);
-        if (e != cudaSuccess) return b2k_fail(ctx, B2K_ECUDA, "gkl_expand_many: %s", cudaGetErrorString(e));
-        B2K_TRY(b2k_stream_sync(ctx));
-        d = enq;
-        for (int32_t i = 0; i < enq; ++i) {
-            const double* r = ctx->h_res + (size_t)B2K_REC * i;
+        const B2kSpace& s = ctx->spaces[sv];
+        fl.rec0 = fr.st; fl.tol = tol; fl.nsteps = enq; fl.ld = s.ld; fl.n = s.n;
+        const int grid = (int)std::max<int64_t>(1, std::min<int64_t>((s.n + 255) / 256, (int64_t)ctx->num_sms * 4));
+        B2K_TRY(fr.enqueue([&]() -> int32_t {
+            b2k_dispatch(ctx, [&](auto t) {
+                using T = decltype(t);
+                k_gkl_flush<T><<<grid, 256, 0, ctx->stream>>>((T*)s.base, fl);
+            });
+            B2K_LAUNCH_CHECK(ctx);
+            return B2K_OK;
+        }));
+        B2K_TRY(fr.fetch(enq));
+        d = fr.count(enq, [&](const double* r) { return gkl_step_stops(r, tol); });
+        for (int32_t i = 0; i < d; ++i) {
+            const double* r = fr.hrec + (size_t)B2K_REC * i;
             alphas_out[i] = r[5];
             betas_out[i] = isfinite(r[5]) ? r[2] : NAN;     // a non-finite alpha stopped the step before its beta
-            if (gkl_step_stops(r, tol)) { d = i + 1; break; }
         }
     } else {
-        cudaStreamSynchronize(ctx->stream);
-    }
-    // column bookkeeping: everything this batch touched is free again, except the d new columns of U and V and the
-    // residual that follows them (steps behind a stop were skipped on the device)
-    for (b2k_vec h : touched) ctx->spaces[B2K_VEC_SPACE(h)].used[B2K_VEC_COL(h)] = 0;
-    if (d > 0) {
-        for (int32_t i = 0; i < d; ++i) {
-            ucols[k + i] = Uh[i];
-            vcols[k + i] = Vh[i];
-            ctx->spaces[su].used[B2K_VEC_COL(Uh[i])] = 1;
-            ctx->spaces[sv].used[B2K_VEC_COL(Vh[i])] = 1;
-        }
-        ucols[k + d] = Wh[d - 1];
-        ctx->spaces[su].used[B2K_VEC_COL(Wh[d - 1])] = 1;
-    } else {
-        ucols[k] = touched[0];                   // nothing ran: r is still r
-        ctx->spaces[su].used[B2K_VEC_COL(touched[0])] = 1;
+        fr.fail(rc);
     }
     *steps_done = d;
-    *r_out = ucols[k + d];
+    *r_out = cc.commit(d, ucols, vcols, k);
     return rc;
 }
 
@@ -2331,8 +2273,7 @@ int32_t lsmr_refuse(b2k_ctx* ctx, const b2k_op* A, const b2k_op* At, const VecRe
     if (krylovdim > 1) {
         if (alg != B2K_MGS && alg != B2K_MGS2 && !gs)
             return b2k_fail(ctx, B2K_ENOTSUP, "lsmr_chain: orthogonalizer %d does not chain with krylovdim > 1", alg);
-        const int C = ctx->dtype == B2K_F64 ? 8 : 16;
-        if (gs && (!g_use_coop || (nring + C - 1) / C > NS || nring > MAXCH * C))
+        if (gs && (!g_use_coop || !ring_holds(ctx->dtype, nring)))
             return b2k_fail(ctx, B2K_ENOTSUP, "lsmr_chain: %d ring columns do not fit the sweep's panel ring", nring);
     }
     if (nring > LS_MAXRING)
@@ -2391,13 +2332,13 @@ extern "C" int32_t b2k_lsmr_chain(b2k_ctx* ctx, const b2k_op* A, const b2k_op* A
     B2K_TRY(lsmr_refuse(ctx, A, At, mv, nv, rr.data(), nring, krylovdim, alg));
     *steps_done = 0;
     const int64_t m = mv[0].n, n = nv[0].n;
-    const bool f64 = ctx->dtype == B2K_F64;
+    B2kChain fr(ctx, LS_NSTATE, LS_REC);
     LsmrDev d;
     memset(&d, 0, sizeof(d));
-    d.st = ctx->d_steps;
-    d.rec0 = ctx->d_steps + LS_NSTATE;
-    d.stop = reinterpret_cast<int*>(ctx->d_sync + B2K_SYNC_STOP);
-    d.skip = reinterpret_cast<int*>(ctx->d_sync + B2K_SYNC_SKIP);
+    d.st = fr.st;
+    d.rec0 = fr.rec0;
+    d.stop = fr.stop;
+    d.skip = fr.skip;
     d.tol = tol;
     d.iter0 = iter0;
     d.nring = nring;
@@ -2406,11 +2347,7 @@ extern "C" int32_t b2k_lsmr_chain(b2k_ctx* ctx, const b2k_op* A, const b2k_op* A
     memcpy(seed, state_in, LS_NIO * sizeof(double));
     seed[LS_INVA] = 1.0;                           // u and v are normalised on entry
     seed[LS_INVB] = 1.0;
-    B2K_TRY(b2k_put_coef(ctx, seed, LS_NSTATE, 0));
-    B2K_CUDA(ctx, cudaMemcpyAsync(d.st, ctx->d_coef, LS_NSTATE * sizeof(double), cudaMemcpyDeviceToDevice, ctx->stream));
-    B2K_CUDA(ctx, cudaMemsetAsync(d.rec0, 0, sizeof(double) * LS_REC * nsteps, ctx->stream));
-    B2K_CUDA(ctx, cudaMemsetAsync(d.stop, 0, sizeof(int), ctx->stream));
-    B2K_CUDA(ctx, cudaMemsetAsync(d.skip, 0, sizeof(int), ctx->stream));
+    B2K_TRY(fr.seed(seed, LS_NSTATE, nsteps, true));
     SpmvFuse fa, ft;
     memset(&fa, 0, sizeof(fa));
     fa.stop = d.stop;
@@ -2419,54 +2356,45 @@ extern "C" int32_t b2k_lsmr_chain(b2k_ctx* ctx, const b2k_op* A, const b2k_op* A
     ft.stop = d.skip;
     ft.xscale = d.st + LS_INVB;
     const bool reorth = krylovdim > 1;
-    int32_t rc = B2K_OK;
-    for (int32_t i = 0; i < nsteps && rc == B2K_OK; ++i) {
-        const int k = iter0 + 1 + i;               // v_k sits (or will sit) in ring slot (k - 1) % nring
-        const VecRef& P = rr[(k - 1) % nring];
-        const VecRef& src = i == 0 ? P : nv[3];
-        const VecRef& yv = i == 0 ? nv[3] : P;
-        if ((rc = b2k_enqueue_apply_fused(ctx, A, src, mv[4], 0.0, 1.0, false, nullptr, nullptr, &fa)) != B2K_OK) break;
-        if ((rc = b2k_lsmr_enqueue_m(ctx, m, mv[0].ptr, mv[1].ptr, mv[2].ptr, mv[3].ptr, mv[4].ptr, i > 0, false, d)) != B2K_OK)
-            break;
-        if ((rc = b2k_enqueue_apply_fused(ctx, At, mv[3], yv, 0.0, 1.0, false, nullptr, nullptr, &ft)) != B2K_OK) break;
-        if ((rc = b2k_lsmr_enqueue_n(ctx, n, nv[0].ptr, nv[1].ptr, nv[2].ptr, P.ptr, nv[3].ptr, i > 0, i > 0, !reorth, d)) !=
-            B2K_OK)
-            break;
-        if (!reorth) continue;
-        const int cnt = std::min(krylovdim, k);    // V holds v_1 .. v_k, at most krylovdim of them, in slot order
-        Panel pn;
-        if ((rc = make_panel(ctx, ring, cnt, &pn)) != B2K_OK) break;
-        if (alg == B2K_MGS || alg == B2K_MGS2) {
-            ctx->dot_stop = d.skip;
-            rc = mgs_sweep(ctx, pn, nv[3], cnt, 0, -1);
-            if (rc == B2K_OK && alg == B2K_MGS2) rc = mgs_sweep(ctx, pn, nv[3], cnt, cnt, -1);
-            ctx->dot_stop = nullptr;
-        } else {                                   // orthogonalize!! with CGS2: two classical passes
-            for (int ps = 0; ps < 2 && rc == B2K_OK; ++ps)
-                rc = f64 ? chain_step_gs<double>(ctx, pn, cnt, nv[3], nullptr, d.st + LS_FIN, -INFINITY, nullptr, false, 0,
-                                                 d.skip)
-                         : chain_step_gs<float>(ctx, pn, cnt, nv[3], nullptr, d.st + LS_FIN, -INFINITY, nullptr, false, 0,
-                                                d.skip);
+    // nothing is reported from a call that could not be enqueued
+    B2K_TRY(fr.enqueue([&]() -> int32_t {
+        for (int32_t i = 0; i < nsteps; ++i) {
+            const int k = iter0 + 1 + i;               // v_k sits (or will sit) in ring slot (k - 1) % nring
+            const VecRef& P = rr[(k - 1) % nring];
+            const VecRef& src = i == 0 ? P : nv[3];
+            const VecRef& yv = i == 0 ? nv[3] : P;
+            B2K_TRY(b2k_enqueue_apply_fused(ctx, A, src, mv[4], 0.0, 1.0, false, nullptr, nullptr, &fa));
+            B2K_TRY(b2k_lsmr_enqueue_m(ctx, m, mv[0].ptr, mv[1].ptr, mv[2].ptr, mv[3].ptr, mv[4].ptr, i > 0, false, d));
+            B2K_TRY(b2k_enqueue_apply_fused(ctx, At, mv[3], yv, 0.0, 1.0, false, nullptr, nullptr, &ft));
+            B2K_TRY(b2k_lsmr_enqueue_n(ctx, n, nv[0].ptr, nv[1].ptr, nv[2].ptr, P.ptr, nv[3].ptr, i > 0, i > 0, !reorth,
+                                       d));
+            if (!reorth) continue;
+            const int cnt = std::min(krylovdim, k);    // V holds v_1 .. v_k, at most krylovdim of them, in slot order
+            Panel pn;
+            B2K_TRY(make_panel(ctx, ring, cnt, &pn));
+            if (alg == B2K_MGS || alg == B2K_MGS2) {
+                ctx->dot_stop = d.skip;
+                int32_t rc = mgs_sweep(ctx, pn, nv[3], cnt, 0, -1);
+                if (rc == B2K_OK && alg == B2K_MGS2) rc = mgs_sweep(ctx, pn, nv[3], cnt, cnt, -1);
+                ctx->dot_stop = nullptr;
+                B2K_TRY(rc);
+            } else {                                   // orthogonalize!! with CGS2: two classical passes
+                for (int ps = 0; ps < 2; ++ps)
+                    B2K_TRY(b2k_dispatch(ctx, [&](auto t) {
+                        return chain_step_gs<decltype(t)>(ctx, pn, cnt, nv[3], nullptr, d.st + LS_FIN, -INFINITY,
+                                                          nullptr, false, 0, d.skip);
+                    }));
+            }
+            B2K_TRY(b2k_lsmr_enqueue_alpha(ctx, n, nv[3].ptr, d));
         }
-        if (rc == B2K_OK) rc = b2k_lsmr_enqueue_alpha(ctx, n, nv[3].ptr, d);
-    }
-    if (rc != B2K_OK) {                            // nothing is reported from a call that could not be enqueued
-        cudaStreamSynchronize(ctx->stream);
-        return rc;
-    }
-    B2K_TRY(b2k_lsmr_enqueue_m(ctx, m, mv[0].ptr, mv[1].ptr, mv[2].ptr, mv[3].ptr, nullptr, true, true, d));
-    B2K_TRY(b2k_lsmr_enqueue_flush_n(ctx, n, nv[0].ptr, nv[1].ptr, nv[2].ptr, nv[3].ptr, d));
-    B2K_CUDA(ctx, cudaMemcpyAsync(ctx->h_res, d.rec0, sizeof(double) * LS_REC * nsteps, cudaMemcpyDeviceToHost,
-                                  ctx->stream));
-    double* hst = ctx->h_res + B2K_RES_DOUBLES - LS_NSTATE / 2;
-    static_assert(LS_NIO <= LS_NSTATE / 2, "state block");
-    B2K_CUDA(ctx, cudaMemcpyAsync(hst, d.st, sizeof(double) * LS_NIO, cudaMemcpyDeviceToHost, ctx->stream));
-    B2K_TRY(b2k_stream_sync(ctx));
-    int32_t dn = nsteps;
-    for (int32_t i = 0; i < nsteps; ++i)
-        if (ctx->h_res[(size_t)LS_REC * i + 7] != 0.0) { dn = i + 1; break; }
-    memcpy(rec_out, ctx->h_res, sizeof(double) * LS_REC * dn);
-    memcpy(state_out, hst, sizeof(double) * LS_NIO);
+        B2K_TRY(b2k_lsmr_enqueue_m(ctx, m, mv[0].ptr, mv[1].ptr, mv[2].ptr, mv[3].ptr, nullptr, true, true, d));
+        return b2k_lsmr_enqueue_flush_n(ctx, n, nv[0].ptr, nv[1].ptr, nv[2].ptr, nv[3].ptr, d);
+    }));
+    static_assert(LS_NIO <= LS_NSTATE, "state block");
+    B2K_TRY(fr.fetch(nsteps, LS_NIO));
+    const int32_t dn = fr.count(nsteps, [](const double* rec) { return rec[7] != 0.0; });
+    memcpy(rec_out, fr.hrec, sizeof(double) * LS_REC * dn);
+    memcpy(state_out, fr.hst, sizeof(double) * LS_NIO);
     *steps_done = dn;
     return B2K_OK;
 }
@@ -2574,12 +2502,10 @@ extern "C" int32_t b2k_basis_rank1update(b2k_ctx* ctx, const b2k_vec* cols, int3
             cf.c[i] = alpha * x_host[off + i];   // real: conj(x) = x
         }
         const int bm = beta == 1.0 ? 1 : (beta == 0.0 ? 0 : 2);
-        if (ctx->dtype == B2K_F64)
-            k_rank1<double><<<grid, 256, 0, ctx->stream>>>((double*)pn.base, pn.ld, pn.n, kk,
-                                                           (const double*)ry.ptr, beta, bm, cl, cf);
-        else
-            k_rank1<float><<<grid, 256, 0, ctx->stream>>>((float*)pn.base, pn.ld, pn.n, kk,
-                                                          (const float*)ry.ptr, (float)beta, bm, cl, cf);
+        b2k_dispatch(ctx, [&](auto t) {
+            using T = decltype(t);
+            k_rank1<T><<<grid, 256, 0, ctx->stream>>>((T*)pn.base, pn.ld, pn.n, kk, (const T*)ry.ptr, T(beta), bm, cl, cf);
+        });
         B2K_LAUNCH_CHECK(ctx);
     }
     return B2K_OK;
@@ -2935,9 +2861,9 @@ extern "C" int32_t b2k_basis_cross_inner(b2k_ctx* ctx, const b2k_vec* X, int32_t
         for (int j0 = 0; rc == B2K_OK && j0 < q; j0 += CI_B) {
             const int pb = std::min(CI_B, p - i0), qb = std::min(CI_B, q - j0);
             if (i0 + pb <= p0 && j0 + qb <= q0) continue;
-            rc = ctx->dtype == B2K_F64
-                     ? cross_block<double>(ctx, xr, yr, i0, pb, j0, qb, p0, q0, n, d_part, d_G, p)
-                     : cross_block<float>(ctx, xr, yr, i0, pb, j0, qb, p0, q0, n, d_part, d_G, p);
+            rc = b2k_dispatch(ctx, [&](auto t) {
+                return cross_block<decltype(t)>(ctx, xr, yr, i0, pb, j0, qb, p0, q0, n, d_part, d_G, p);
+            });
         }
     if (rc == B2K_OK) {
         const cudaError_t e = cudaMemcpyAsync(h_G, d_G, sizeof(double) * (size_t)p * q, cudaMemcpyDeviceToHost,

@@ -1000,17 +1000,13 @@ k_lsmr_flush_n(T* __restrict__ x, T* __restrict__ h, T* __restrict__ hb, T* spar
 int32_t b2k_lsmr_enqueue_m(b2k_ctx* ctx, int64_t m, void* r, void* Ah, void* Ahbar, void* u, const void* Av,
                            bool pend, bool flush, const LsmrDev& d) {
     const int grid = grid_for(ctx, m, 4);
-#define LAUNCH(T, FL)                                                                                               \
-    k_lsmr_m<T, FL><<<grid, BT, 0, ctx->stream>>>((T*)r, (T*)Ah, (T*)Ahbar, (T*)u, (const T*)Av, m, pend,         \
-                                                  ctx->d_part_s, ctx->d_sync, d)
-    if (ctx->dtype == B2K_F64) {
-        if (flush) LAUNCH(double, true);
-        else LAUNCH(double, false);
-    } else {
-        if (flush) LAUNCH(float, true);
-        else LAUNCH(float, false);
-    }
-#undef LAUNCH
+    b2k_dispatch(ctx, [&](auto t) {
+        using T = decltype(t);
+        b2k_flag(flush, [&](auto fl) {
+            k_lsmr_m<T, fl><<<grid, BT, 0, ctx->stream>>>((T*)r, (T*)Ah, (T*)Ahbar, (T*)u, (const T*)Av, m, pend,
+                                                          ctx->d_part_s, ctx->d_sync, d);
+        });
+    });
     B2K_LAUNCH_CHECK(ctx);
     return B2K_OK;
 }
@@ -1018,27 +1014,23 @@ int32_t b2k_lsmr_enqueue_m(b2k_ctx* ctx, int64_t m, void* r, void* Ah, void* Ahb
 int32_t b2k_lsmr_enqueue_n(b2k_ctx* ctx, int64_t n, void* x, void* h, void* hbar, void* P, void* Q, bool swap,
                            bool pend, bool norm, const LsmrDev& d) {
     const int grid = grid_for(ctx, n, 4);
-#define LAUNCH(T, NR)                                                                                               \
-    k_lsmr_n<T, NR><<<grid, BT, 0, ctx->stream>>>((T*)x, (T*)h, (T*)hbar, (T*)P, (T*)Q, n, swap, pend,            \
-                                                  ctx->d_part_s, ctx->d_sync, d)
-    if (ctx->dtype == B2K_F64) {
-        if (norm) LAUNCH(double, true);
-        else LAUNCH(double, false);
-    } else {
-        if (norm) LAUNCH(float, true);
-        else LAUNCH(float, false);
-    }
-#undef LAUNCH
+    b2k_dispatch(ctx, [&](auto t) {
+        using T = decltype(t);
+        b2k_flag(norm, [&](auto nr) {
+            k_lsmr_n<T, nr><<<grid, BT, 0, ctx->stream>>>((T*)x, (T*)h, (T*)hbar, (T*)P, (T*)Q, n, swap, pend,
+                                                          ctx->d_part_s, ctx->d_sync, d);
+        });
+    });
     B2K_LAUNCH_CHECK(ctx);
     return B2K_OK;
 }
 
 int32_t b2k_lsmr_enqueue_alpha(b2k_ctx* ctx, int64_t n, const void* Q, const LsmrDev& d) {
     const int grid = grid_for(ctx, n, 8);
-    if (ctx->dtype == B2K_F64)
-        k_lsmr_alpha<double><<<grid, BT, 0, ctx->stream>>>((const double*)Q, n, ctx->d_part_s, ctx->d_sync, d);
-    else
-        k_lsmr_alpha<float><<<grid, BT, 0, ctx->stream>>>((const float*)Q, n, ctx->d_part_s, ctx->d_sync, d);
+    b2k_dispatch(ctx, [&](auto t) {
+        using T = decltype(t);
+        k_lsmr_alpha<T><<<grid, BT, 0, ctx->stream>>>((const T*)Q, n, ctx->d_part_s, ctx->d_sync, d);
+    });
     B2K_LAUNCH_CHECK(ctx);
     return B2K_OK;
 }
@@ -1046,10 +1038,10 @@ int32_t b2k_lsmr_enqueue_alpha(b2k_ctx* ctx, int64_t n, const void* Q, const Lsm
 int32_t b2k_lsmr_enqueue_flush_n(b2k_ctx* ctx, int64_t n, void* x, void* h, void* hbar, void* spare,
                                  const LsmrDev& d) {
     const int grid = grid_for(ctx, n, 4);
-    if (ctx->dtype == B2K_F64)
-        k_lsmr_flush_n<double><<<grid, BT, 0, ctx->stream>>>((double*)x, (double*)h, (double*)hbar, (double*)spare, n, d);
-    else
-        k_lsmr_flush_n<float><<<grid, BT, 0, ctx->stream>>>((float*)x, (float*)h, (float*)hbar, (float*)spare, n, d);
+    b2k_dispatch(ctx, [&](auto t) {
+        using T = decltype(t);
+        k_lsmr_flush_n<T><<<grid, BT, 0, ctx->stream>>>((T*)x, (T*)h, (T*)hbar, (T*)spare, n, d);
+    });
     B2K_LAUNCH_CHECK(ctx);
     return B2K_OK;
 }
@@ -1065,43 +1057,30 @@ int32_t b2k_enqueue_dot(b2k_ctx* ctx, const void* q, void* x, int64_t n, const v
     double* acc = accum_slot >= 0 ? ctx->d_res + accum_slot : nullptr;
     const double* sp = sprev_slot >= 0 ? ctx->d_res + sprev_slot : nullptr;
     unsigned* ticket = ctx->d_sync;
-#define LAUNCH_S(T, UPD, NRM, ST)                                                                    \
-    k_dot<T, UPD, NRM, ST><<<grid, BT, 0, ctx->stream>>>((const T*)q, (T*)x, n, (const T*)qprev, sp,         \
-                                                         ctx->d_part_s, ticket, out, acc, ctx->dot_hints,   \
-                                                         ctx->dot_stop)
-#define LAUNCH(T, UPD, NRM)                          \
-    do {                                             \
-        if (ctx->dot_stop) LAUNCH_S(T, UPD, NRM, true); \
-        else LAUNCH_S(T, UPD, NRM, false);           \
-    } while (0)
-    const bool upd = qprev != nullptr, nrm = q == nullptr;
-    if (ctx->dtype == B2K_F64) {
-        if (upd && nrm) LAUNCH(double, true, true);
-        else if (upd) LAUNCH(double, true, false);
-        else if (nrm) LAUNCH(double, false, true);
-        else LAUNCH(double, false, false);
-    } else {
-        if (upd && nrm) LAUNCH(float, true, true);
-        else if (upd) LAUNCH(float, true, false);
-        else if (nrm) LAUNCH(float, false, true);
-        else LAUNCH(float, false, false);
-    }
-#undef LAUNCH
-#undef LAUNCH_S
+    b2k_dispatch(ctx, [&](auto t) {
+        using T = decltype(t);
+        b2k_flag(qprev != nullptr, [&](auto upd) {
+            b2k_flag(q == nullptr, [&](auto nrm) {
+                b2k_flag(ctx->dot_stop != nullptr, [&](auto st) {
+                    k_dot<T, upd, nrm, st><<<grid, BT, 0, ctx->stream>>>((const T*)q, (T*)x, n, (const T*)qprev, sp,
+                                                                         ctx->d_part_s, ticket, out, acc,
+                                                                         ctx->dot_hints, ctx->dot_stop);
+                });
+            });
+        });
+    });
     B2K_LAUNCH_CHECK(ctx);
     return B2K_OK;
 }
 
 int32_t b2k_enqueue_axpy_dev(b2k_ctx* ctx, void* x, const void* q, int s_slot, int64_t n) {
     const int grid = grid_for(ctx, n, 8);
-    const int* st = ctx->dot_stop;
-    if (ctx->dtype == B2K_F64) {
-        if (st) k_axpy_dev<double, true><<<grid, BT, 0, ctx->stream>>>((double*)x, (const double*)q, ctx->d_res + s_slot, n, st);
-        else k_axpy_dev<double><<<grid, BT, 0, ctx->stream>>>((double*)x, (const double*)q, ctx->d_res + s_slot, n, st);
-    } else {
-        if (st) k_axpy_dev<float, true><<<grid, BT, 0, ctx->stream>>>((float*)x, (const float*)q, ctx->d_res + s_slot, n, st);
-        else k_axpy_dev<float><<<grid, BT, 0, ctx->stream>>>((float*)x, (const float*)q, ctx->d_res + s_slot, n, st);
-    }
+    b2k_dispatch(ctx, [&](auto t) {
+        using T = decltype(t);
+        b2k_flag(ctx->dot_stop != nullptr, [&](auto st) {
+            k_axpy_dev<T, st><<<grid, BT, 0, ctx->stream>>>((T*)x, (const T*)q, ctx->d_res + s_slot, n, ctx->dot_stop);
+        });
+    });
     B2K_LAUNCH_CHECK(ctx);
     return B2K_OK;
 }
@@ -1115,10 +1094,10 @@ extern "C" int32_t b2k_vec_fill_splitmix(b2k_ctx* ctx, b2k_vec v, uint64_t seed)
     if (r.n == 0) return B2K_OK;
     const int grid = grid_for(ctx, r.n, 4);
     const uint64_t off = r.sharded ? (uint64_t)ctx->row_offset : 0ull;
-    if (ctx->dtype == B2K_F64)
-        k_fill_splitmix<double><<<grid, BT, 0, ctx->stream>>>((double*)r.ptr, r.n, seed, off);
-    else
-        k_fill_splitmix<float><<<grid, BT, 0, ctx->stream>>>((float*)r.ptr, r.n, seed, off);
+    b2k_dispatch(ctx, [&](auto t) {
+        using T = decltype(t);
+        k_fill_splitmix<T><<<grid, BT, 0, ctx->stream>>>((T*)r.ptr, r.n, seed, off);
+    });
     B2K_LAUNCH_CHECK(ctx);
     return B2K_OK;
 }
@@ -1129,61 +1108,50 @@ extern "C" int32_t b2k_vec_fill(b2k_ctx* ctx, b2k_vec v, double value) {
     B2K_TRY(b2k_resolve(ctx, v, &r));
     if (r.n == 0) return B2K_OK;
     const int grid = grid_for(ctx, r.n, 4);
-    if (ctx->dtype == B2K_F64)
-        k_fill<double><<<grid, BT, 0, ctx->stream>>>((double*)r.ptr, r.n, value);
-    else
-        k_fill<float><<<grid, BT, 0, ctx->stream>>>((float*)r.ptr, r.n, (float)value);
+    b2k_dispatch(ctx, [&](auto t) {
+        using T = decltype(t);
+        k_fill<T><<<grid, BT, 0, ctx->stream>>>((T*)r.ptr, r.n, T(value));
+    });
     B2K_LAUNCH_CHECK(ctx);
     return B2K_OK;
 }
 
 extern "C" int32_t b2k_vec_scale(b2k_ctx* ctx, b2k_vec y, b2k_vec x, double alpha) {
     if (!ctx) return B2K_EINVAL;
-    VecRef ry, rx;
-    B2K_TRY(b2k_resolve(ctx, y, &ry));
-    B2K_TRY(b2k_resolve(ctx, x, &rx));
-    if (ry.n != rx.n) return b2k_fail(ctx, B2K_EDIM, "vec_scale: length mismatch");
+    VecRef v[2];
+    B2K_TRY(b2k_resolve_vecs(ctx, "vec_scale", {y, x}, v));
+    const VecRef &ry = v[0], &rx = v[1];
     if (ry.n == 0) return B2K_OK;
     const int grid = grid_for(ctx, ry.n, 8);
-    if (ctx->dtype == B2K_F64)
-        k_scale<double><<<grid, BT, 0, ctx->stream>>>((double*)ry.ptr, (const double*)rx.ptr,
-                                                      ry.n, alpha);
-    else
-        k_scale<float><<<grid, BT, 0, ctx->stream>>>((float*)ry.ptr, (const float*)rx.ptr, ry.n,
-                                                     (float)alpha);
+    b2k_dispatch(ctx, [&](auto t) {
+        using T = decltype(t);
+        k_scale<T><<<grid, BT, 0, ctx->stream>>>((T*)ry.ptr, (const T*)rx.ptr, ry.n, T(alpha));
+    });
     B2K_LAUNCH_CHECK(ctx);
     return B2K_OK;
 }
 
 extern "C" int32_t b2k_vec_axpby(b2k_ctx* ctx, b2k_vec y, b2k_vec x, double alpha, double beta) {
     if (!ctx) return B2K_EINVAL;
-    VecRef ry, rx;
-    B2K_TRY(b2k_resolve(ctx, y, &ry));
-    B2K_TRY(b2k_resolve(ctx, x, &rx));
-    if (ry.n != rx.n) return b2k_fail(ctx, B2K_EDIM, "vec_axpby: length mismatch");
+    VecRef v[2];
+    B2K_TRY(b2k_resolve_vecs(ctx, "vec_axpby", {y, x}, v));
+    const VecRef &ry = v[0], &rx = v[1];
     if (ry.n == 0) return B2K_OK;
     // add!!(y, y, alpha, beta): y <- (beta + alpha) * y would change rounding; do it literally, reading y once
     const bool self = ry.ptr == rx.ptr;
     const int grid = grid_for(ctx, ry.n, 8);
-#define LAUNCH_S(T, MODE, SELF)                                                                              \
-    k_axpby<T, MODE, SELF><<<grid, BT, 0, ctx->stream>>>((T*)ry.ptr, SELF ? nullptr : (const T*)rx.ptr, ry.n, \
-                                                         (T)alpha, (T)beta)
-#define LAUNCH(T, MODE)                       \
-    do {                                      \
-        if (self) LAUNCH_S(T, MODE, true);    \
-        else LAUNCH_S(T, MODE, false);        \
-    } while (0)
-    if (ctx->dtype == B2K_F64) {
-        if (beta == 0.0) LAUNCH(double, 0);
-        else if (beta == 1.0) LAUNCH(double, 1);
-        else LAUNCH(double, 2);
-    } else {
-        if (beta == 0.0) LAUNCH(float, 0);
-        else if (beta == 1.0) LAUNCH(float, 1);
-        else LAUNCH(float, 2);
-    }
-#undef LAUNCH
-#undef LAUNCH_S
+    b2k_dispatch(ctx, [&](auto t) {
+        using T = decltype(t);
+        b2k_flag(self, [&](auto sf) {
+            auto launch = [&](auto mode) {
+                k_axpby<T, mode, sf><<<grid, BT, 0, ctx->stream>>>((T*)ry.ptr, sf ? nullptr : (const T*)rx.ptr,
+                                                                   ry.n, T(alpha), T(beta));
+            };
+            if (beta == 0.0) launch(std::integral_constant<int, 0>());
+            else if (beta == 1.0) launch(std::integral_constant<int, 1>());
+            else launch(std::integral_constant<int, 2>());
+        });
+    });
     B2K_LAUNCH_CHECK(ctx);
     return B2K_OK;
 }
@@ -1191,50 +1159,42 @@ extern "C" int32_t b2k_vec_axpby(b2k_ctx* ctx, b2k_vec y, b2k_vec x, double alph
 extern "C" int32_t b2k_vec_axpy2(b2k_ctx* ctx, b2k_vec y, b2k_vec x1, double a1, b2k_vec x2,
                                  double a2) {
     if (!ctx) return B2K_EINVAL;
-    VecRef ry, r1, r2;
-    B2K_TRY(b2k_resolve(ctx, y, &ry));
-    B2K_TRY(b2k_resolve(ctx, x1, &r1));
-    B2K_TRY(b2k_resolve(ctx, x2, &r2));
-    if (ry.n != r1.n || ry.n != r2.n) return b2k_fail(ctx, B2K_EDIM, "vec_axpy2: length mismatch");
+    VecRef v[3];
+    B2K_TRY(b2k_resolve_vecs(ctx, "vec_axpy2", {y, x1, x2}, v));
+    const VecRef &ry = v[0], &r1 = v[1], &r2 = v[2];
     if (ry.ptr == r1.ptr || ry.ptr == r2.ptr)
         return b2k_fail(ctx, B2K_EINVAL, "vec_axpy2: y must not alias x1/x2");
     if (ry.n == 0) return B2K_OK;
     const int grid = grid_for(ctx, ry.n, 8);
-    if (ctx->dtype == B2K_F64)
-        k_axpy2<double><<<grid, BT, 0, ctx->stream>>>((double*)ry.ptr, (const double*)r1.ptr, a1,
-                                                      (const double*)r2.ptr, a2, ry.n);
-    else
-        k_axpy2<float><<<grid, BT, 0, ctx->stream>>>((float*)ry.ptr, (const float*)r1.ptr,
-                                                     (float)a1, (const float*)r2.ptr, (float)a2,
-                                                     ry.n);
+    b2k_dispatch(ctx, [&](auto t) {
+        using T = decltype(t);
+        k_axpy2<T><<<grid, BT, 0, ctx->stream>>>((T*)ry.ptr, (const T*)r1.ptr, T(a1), (const T*)r2.ptr, T(a2), ry.n);
+    });
     B2K_LAUNCH_CHECK(ctx);
     return B2K_OK;
 }
 
 extern "C" int32_t b2k_basis_givens(b2k_ctx* ctx, b2k_vec q1, b2k_vec q2, double c, double s) {
     if (!ctx) return B2K_EINVAL;
-    VecRef r1, r2;
-    B2K_TRY(b2k_resolve(ctx, q1, &r1));
-    B2K_TRY(b2k_resolve(ctx, q2, &r2));
-    if (r1.n != r2.n) return b2k_fail(ctx, B2K_EDIM, "basis_givens: length mismatch");
+    VecRef v[2];
+    B2K_TRY(b2k_resolve_vecs(ctx, "basis_givens", {q1, q2}, v));
+    const VecRef &r1 = v[0], &r2 = v[1];
     if (r1.ptr == r2.ptr) return b2k_fail(ctx, B2K_EINVAL, "basis_givens: q1 == q2");
     if (r1.n == 0) return B2K_OK;
     const int grid = grid_for(ctx, r1.n, 8);
-    if (ctx->dtype == B2K_F64)
-        k_givens<double><<<grid, BT, 0, ctx->stream>>>((double*)r1.ptr, (double*)r2.ptr, r1.n, c, s);
-    else
-        k_givens<float><<<grid, BT, 0, ctx->stream>>>((float*)r1.ptr, (float*)r2.ptr, r1.n,
-                                                      (float)c, (float)s);
+    b2k_dispatch(ctx, [&](auto t) {
+        using T = decltype(t);
+        k_givens<T><<<grid, BT, 0, ctx->stream>>>((T*)r1.ptr, (T*)r2.ptr, r1.n, T(c), T(s));
+    });
     B2K_LAUNCH_CHECK(ctx);
     return B2K_OK;
 }
 
 extern "C" int32_t b2k_vec_inner(b2k_ctx* ctx, b2k_vec x, b2k_vec y, double* out) {
     if (!ctx || !out) return B2K_EINVAL;
-    VecRef rx, ry;
-    B2K_TRY(b2k_resolve(ctx, x, &rx));
-    B2K_TRY(b2k_resolve(ctx, y, &ry));
-    if (rx.n != ry.n) return b2k_fail(ctx, B2K_EDIM, "vec_inner: length mismatch");
+    VecRef v[2];
+    B2K_TRY(b2k_resolve_vecs(ctx, "vec_inner", {x, y}, v));
+    const VecRef &rx = v[0], &ry = v[1];
     B2K_TRY(b2k_enqueue_dot(ctx, rx.ptr, ry.ptr, rx.n, nullptr, -1, 0, -1));
     B2K_TRY(b2k_fetch_results(ctx, 1, rx.sharded));
     *out = ctx->h_res[0];
@@ -1255,10 +1215,9 @@ extern "C" int32_t b2k_vec_norm(b2k_ctx* ctx, b2k_vec x, double* out) {
 extern "C" int32_t b2k_vec_orthogonalize(b2k_ctx* ctx, b2k_vec v, b2k_vec q, int32_t alg,
                                          double eta, double* s_out, double* nrm_out) {
     if (!ctx || !s_out) return B2K_EINVAL;
-    VecRef rv, rq;
-    B2K_TRY(b2k_resolve(ctx, v, &rv));
-    B2K_TRY(b2k_resolve(ctx, q, &rq));
-    if (rv.n != rq.n) return b2k_fail(ctx, B2K_EDIM, "vec_orthogonalize: length mismatch");
+    VecRef vq[2];
+    B2K_TRY(b2k_resolve_vecs(ctx, "vec_orthogonalize", {v, q}, vq));
+    const VecRef &rv = vq[0], &rq = vq[1];
     if (rv.ptr == rq.ptr) return b2k_fail(ctx, B2K_EINVAL, "vec_orthogonalize: v == q");
     const int64_t n = rv.n;
     const int sh = rv.sharded;
@@ -1297,7 +1256,7 @@ extern "C" int32_t b2k_vec_orthogonalize(b2k_ctx* ctx, b2k_vec v, b2k_vec q, int
         double nold = sqrt(ctx->h_res[1]);
         s = ctx->h_res[0];
         double nnew = sqrt(ctx->h_res[2]);
-        const double eps = (ctx->dtype == B2K_F64) ? 0x1p-52 : 0x1p-23;    // eps(T), orthonormal.jl:481
+        const double eps = b2k_eps(ctx);
         while (eps < nnew && nnew < eta * nold) {
             nold = nnew;
             B2K_TRY(dot(0));
@@ -1329,25 +1288,19 @@ extern "C" int32_t b2k_cg_step(b2k_ctx* ctx, const b2k_op* op, b2k_vec x, b2k_ve
                                double a0, double a1, double beta, double rho, double* pq_out,
                                double* normr_out) {
     if (!ctx || !op || !pq_out || !normr_out) return B2K_EINVAL;
-    VecRef rx, rr, rp, rq;
-    B2K_TRY(b2k_resolve(ctx, x, &rx));
-    B2K_TRY(b2k_resolve(ctx, r, &rr));
-    B2K_TRY(b2k_resolve(ctx, p, &rp));
-    B2K_TRY(b2k_resolve(ctx, q, &rq));
-    if (rx.n != rr.n || rx.n != rp.n || rx.n != rq.n) return b2k_fail(ctx, B2K_EDIM, "cg_step: length mismatch");
+    VecRef v[4];
+    B2K_TRY(b2k_resolve_vecs(ctx, "cg_step", {x, r, p, q}, v));
+    const VecRef &rx = v[0], &rr = v[1], &rp = v[2], &rq = v[3];
     B2K_TRY(b2k_vec_axpby(ctx, p, r, 1.0, beta));
     const bool shifted = (a0 != 0.0) || (a1 != 1.0);
     B2K_TRY(b2k_enqueue_apply(ctx, op, rp, rq, a0, a1, shifted, &rp, 0));
     B2K_TRY(b2k_allreduce(ctx, ctx->d_res, 1, rp.sharded));
     const int grid = grid_for(ctx, rx.n, 8);
-    if (ctx->dtype == B2K_F64)
-        k_cg_xr<double><<<grid, BT, 0, ctx->stream>>>((double*)rx.ptr, (double*)rr.ptr, (const double*)rp.ptr,
-                                                      (const double*)rq.ptr, rx.n, rho, ctx->d_res,
-                                                      ctx->d_part_s, ctx->d_sync, ctx->d_res + 1, CgChain{});
-    else
-        k_cg_xr<float><<<grid, BT, 0, ctx->stream>>>((float*)rx.ptr, (float*)rr.ptr, (const float*)rp.ptr,
-                                                     (const float*)rq.ptr, rx.n, rho, ctx->d_res,
-                                                     ctx->d_part_s, ctx->d_sync, ctx->d_res + 1, CgChain{});
+    b2k_dispatch(ctx, [&](auto t) {
+        using T = decltype(t);
+        k_cg_xr<T><<<grid, BT, 0, ctx->stream>>>((T*)rx.ptr, (T*)rr.ptr, (const T*)rp.ptr, (const T*)rq.ptr, rx.n, rho,
+                                                 ctx->d_res, ctx->d_part_s, ctx->d_sync, ctx->d_res + 1, CgChain{});
+    });
     B2K_LAUNCH_CHECK(ctx);
     B2K_TRY(b2k_allreduce(ctx, ctx->d_res + 1, 1, rx.sharded));
     B2K_TRY(b2k_fetch_results(ctx, 2, 0));
@@ -1368,56 +1321,46 @@ extern "C" int32_t b2k_cg_chain(b2k_ctx* ctx, const b2k_op* op, b2k_vec x, b2k_v
     if (!ctx || !op || !pq_out || !normr_out || !steps_done || nsteps < 1) return B2K_EINVAL;
     *steps_done = 0;
     if (nsteps > B2K_MAX_CHAIN) nsteps = B2K_MAX_CHAIN;
-    VecRef rx, rr, rp, rq;
-    B2K_TRY(b2k_resolve(ctx, x, &rx));
-    B2K_TRY(b2k_resolve(ctx, r, &rr));
-    B2K_TRY(b2k_resolve(ctx, p, &rp));
-    B2K_TRY(b2k_resolve(ctx, q, &rq));
-    if (rx.n != rr.n || rx.n != rp.n || rx.n != rq.n) return b2k_fail(ctx, B2K_EDIM, "cg_chain: length mismatch");
+    VecRef v[4];
+    B2K_TRY(b2k_resolve_vecs(ctx, "cg_chain", {x, r, p, q}, v, true));
+    const VecRef &rx = v[0], &rr = v[1], &rp = v[2], &rq = v[3];
     if (ctx->nranks > 1) return b2k_fail(ctx, B2K_ENOTSUP, "cg_chain: single-GPU contexts (use b2k_cg_step)");
     int64_t orows = 0, ocols = 0;
     int32_t okind = -1;
     B2K_TRY(b2k_op_info(op, &orows, &ocols, nullptr, &okind));
     if (okind != 0) return b2k_fail(ctx, B2K_ENOTSUP, "cg_chain: CSR operators only");
-    double* state = ctx->d_steps;                       // {rho, beta}
-    double* rec0 = ctx->d_steps + B2K_REC;
-    int* d_stop = reinterpret_cast<int*>(ctx->d_sync + B2K_SYNC_STOP);
+    B2kChain fr(ctx, B2K_REC);                          // state {rho, beta}
     const double seed[2] = {rho, beta};
-    B2K_TRY(b2k_put_coef(ctx, seed, 2, 0));
-    B2K_CUDA(ctx, cudaMemcpyAsync(state, ctx->d_coef, 2 * sizeof(double), cudaMemcpyDeviceToDevice, ctx->stream));
-    B2K_CUDA(ctx, cudaMemsetAsync(d_stop, 0, sizeof(int), ctx->stream));
+    B2K_TRY(fr.seed(seed, 2, 0));
     const bool shifted = (a0 != 0.0) || (a1 != 1.0);
     const int grid = grid_for(ctx, rx.n, 8);
-    for (int32_t i = 0; i < nsteps; ++i) {
-        double* rec = rec0 + (size_t)B2K_REC * i;
-        if (ctx->dtype == B2K_F64)
-            k_xpby_dev<double><<<grid, BT, 0, ctx->stream>>>((double*)rp.ptr, (const double*)rr.ptr, rx.n, state + 1, d_stop);
-        else
-            k_xpby_dev<float><<<grid, BT, 0, ctx->stream>>>((float*)rp.ptr, (const float*)rr.ptr, rx.n, state + 1, d_stop);
-        B2K_LAUNCH_CHECK(ctx);
-        SpmvFuse fz;
-        memset(&fz, 0, sizeof(fz));
-        fz.stop = d_stop;
-        B2K_TRY(b2k_enqueue_apply_fused(ctx, op, rp, rq, a0, a1, shifted, &rp, ctx->d_res, &fz));
-        CgChain ch;
-        ch.state = state; ch.rec = rec; ch.stop = d_stop; ch.tol = tol;
-        if (ctx->dtype == B2K_F64)
-            k_cg_xr<double><<<grid, BT, 0, ctx->stream>>>((double*)rx.ptr, (double*)rr.ptr, (const double*)rp.ptr,
-                                                          (const double*)rq.ptr, rx.n, 0.0, ctx->d_res,
-                                                          ctx->d_part_s, ctx->d_sync, ctx->d_res + 1, ch);
-        else
-            k_cg_xr<float><<<grid, BT, 0, ctx->stream>>>((float*)rx.ptr, (float*)rr.ptr, (const float*)rp.ptr,
-                                                         (const float*)rq.ptr, rx.n, 0.0, ctx->d_res,
-                                                         ctx->d_part_s, ctx->d_sync, ctx->d_res + 1, ch);
-        B2K_LAUNCH_CHECK(ctx);
-    }
-    B2K_CUDA(ctx, cudaMemcpyAsync(ctx->h_res, rec0, sizeof(double) * B2K_REC * nsteps, cudaMemcpyDeviceToHost, ctx->stream));
-    B2K_TRY(b2k_stream_sync(ctx));
-    int32_t d = nsteps;
-    for (int32_t i = 0; i < nsteps; ++i) {
-        pq_out[i] = ctx->h_res[(size_t)B2K_REC * i];
-        normr_out[i] = ctx->h_res[(size_t)B2K_REC * i + 1];
-        if (normr_out[i] < tol) { d = i + 1; break; }
+    B2K_TRY(fr.enqueue([&]() -> int32_t {
+        for (int32_t i = 0; i < nsteps; ++i) {
+            const CgChain ch{fr.st, fr.rec0 + (size_t)B2K_REC * i, fr.stop, tol};
+            b2k_dispatch(ctx, [&](auto t) {
+                using T = decltype(t);
+                k_xpby_dev<T><<<grid, BT, 0, ctx->stream>>>((T*)rp.ptr, (const T*)rr.ptr, rx.n, fr.st + 1, fr.stop);
+            });
+            B2K_LAUNCH_CHECK(ctx);
+            SpmvFuse fz;
+            memset(&fz, 0, sizeof(fz));
+            fz.stop = fr.stop;
+            B2K_TRY(b2k_enqueue_apply_fused(ctx, op, rp, rq, a0, a1, shifted, &rp, ctx->d_res, &fz));
+            b2k_dispatch(ctx, [&](auto t) {
+                using T = decltype(t);
+                k_cg_xr<T><<<grid, BT, 0, ctx->stream>>>((T*)rx.ptr, (T*)rr.ptr, (const T*)rp.ptr, (const T*)rq.ptr,
+                                                         rx.n, 0.0, ctx->d_res, ctx->d_part_s, ctx->d_sync,
+                                                         ctx->d_res + 1, ch);
+            });
+            B2K_LAUNCH_CHECK(ctx);
+        }
+        return B2K_OK;
+    }));
+    B2K_TRY(fr.fetch(nsteps));
+    const int32_t d = fr.count(nsteps, [&](const double* rec) { return rec[1] < tol; });
+    for (int32_t i = 0; i < d; ++i) {
+        pq_out[i] = fr.hrec[(size_t)B2K_REC * i];
+        normr_out[i] = fr.hrec[(size_t)B2K_REC * i + 1];
     }
     *steps_done = d;
     return B2K_OK;
@@ -1433,38 +1376,29 @@ extern "C" int32_t b2k_bicgstab_half(b2k_ctx* ctx, const b2k_op* op, b2k_vec rs,
                                      b2k_vec s, double a0, double a1, double beta, double omega, double rho,
                                      int32_t first, double* sigma_out, double* norms_out) {
     if (!ctx || !op || !sigma_out || !norms_out) return B2K_EINVAL;
-    VecRef rrs, rr, rp, rv, rsv;
-    B2K_TRY(b2k_resolve(ctx, rs, &rrs));
-    B2K_TRY(b2k_resolve(ctx, r, &rr));
-    B2K_TRY(b2k_resolve(ctx, p, &rp));
-    B2K_TRY(b2k_resolve(ctx, v, &rv));
-    B2K_TRY(b2k_resolve(ctx, s, &rsv));
+    VecRef vr[5];
+    B2K_TRY(b2k_resolve_vecs(ctx, "bicgstab_half", {rs, r, p, v, s}, vr));
+    const VecRef &rrs = vr[0], &rr = vr[1], &rp = vr[2], &rv = vr[3], &rsv = vr[4];
     const int64_t n = rr.n;
-    if (rrs.n != n || rp.n != n || rv.n != n || rsv.n != n)
-        return b2k_fail(ctx, B2K_EDIM, "bicgstab_half: length mismatch");
     const int grid = grid_for(ctx, n, 8);
     if (first) {
         B2K_TRY(b2k_vec_copy(ctx, p, r));
-    } else if (ctx->dtype == B2K_F64) {
-        k_bicg_p<double><<<grid, BT, 0, ctx->stream>>>((double*)rp.ptr, (const double*)rr.ptr,
-                                                       (const double*)rv.ptr, n, beta, omega, BicgChain{});
-        B2K_LAUNCH_CHECK(ctx);
     } else {
-        k_bicg_p<float><<<grid, BT, 0, ctx->stream>>>((float*)rp.ptr, (const float*)rr.ptr, (const float*)rv.ptr,
-                                                      n, (float)beta, (float)omega, BicgChain{});
+        b2k_dispatch(ctx, [&](auto t) {
+            using T = decltype(t);
+            k_bicg_p<T><<<grid, BT, 0, ctx->stream>>>((T*)rp.ptr, (const T*)rr.ptr, (const T*)rv.ptr, n, T(beta),
+                                                      T(omega), BicgChain{});
+        });
         B2K_LAUNCH_CHECK(ctx);
     }
     const bool shifted = (a0 != 0.0) || (a1 != 1.0);
     B2K_TRY(b2k_enqueue_apply(ctx, op, rp, rv, a0, a1, shifted, &rrs, 0));      // d_res[0] = sigma
     B2K_TRY(b2k_allreduce(ctx, ctx->d_res, 1, rr.sharded));
-    if (ctx->dtype == B2K_F64)
-        k_bicg_s<double><<<grid, BT, 0, ctx->stream>>>((double*)rsv.ptr, (const double*)rr.ptr,
-                                                       (const double*)rv.ptr, n, rho, ctx->d_res, ctx->d_part_s,
-                                                       ctx->d_sync, ctx->d_res + 1, BicgChain{});
-    else
-        k_bicg_s<float><<<grid, BT, 0, ctx->stream>>>((float*)rsv.ptr, (const float*)rr.ptr, (const float*)rv.ptr,
-                                                      n, rho, ctx->d_res, ctx->d_part_s, ctx->d_sync,
-                                                      ctx->d_res + 1, BicgChain{});
+    b2k_dispatch(ctx, [&](auto t) {
+        using T = decltype(t);
+        k_bicg_s<T><<<grid, BT, 0, ctx->stream>>>((T*)rsv.ptr, (const T*)rr.ptr, (const T*)rv.ptr, n, rho, ctx->d_res,
+                                                  ctx->d_part_s, ctx->d_sync, ctx->d_res + 1, BicgChain{});
+    });
     B2K_LAUNCH_CHECK(ctx);
     B2K_TRY(b2k_allreduce(ctx, ctx->d_res + 1, 1, rr.sharded));
     B2K_TRY(b2k_fetch_results(ctx, 2, 0));
@@ -1477,33 +1411,22 @@ extern "C" int32_t b2k_bicgstab_full(b2k_ctx* ctx, const b2k_op* op, b2k_vec x, 
                                      b2k_vec s, b2k_vec t, double a0, double a1, double alpha,
                                      double* omega_out, double* normr_out, double* rho_out) {
     if (!ctx || !op || !omega_out || !normr_out || !rho_out) return B2K_EINVAL;
-    VecRef rx, rr, rrs, rp, rsv, rt;
-    B2K_TRY(b2k_resolve(ctx, x, &rx));
-    B2K_TRY(b2k_resolve(ctx, r, &rr));
-    B2K_TRY(b2k_resolve(ctx, rs, &rrs));
-    B2K_TRY(b2k_resolve(ctx, p, &rp));
-    B2K_TRY(b2k_resolve(ctx, s, &rsv));
-    B2K_TRY(b2k_resolve(ctx, t, &rt));
+    VecRef vr[6];
+    B2K_TRY(b2k_resolve_vecs(ctx, "bicgstab_full", {x, r, rs, p, s, t}, vr));
+    const VecRef &rx = vr[0], &rr = vr[1], &rrs = vr[2], &rp = vr[3], &rsv = vr[4], &rt = vr[5];
     const int64_t n = rr.n;
-    if (rx.n != n || rrs.n != n || rp.n != n || rsv.n != n || rt.n != n)
-        return b2k_fail(ctx, B2K_EDIM, "bicgstab_full: length mismatch");
     const bool shifted = (a0 != 0.0) || (a1 != 1.0);
     B2K_TRY(b2k_enqueue_apply(ctx, op, rsv, rt, a0, a1, shifted, &rsv, 0));     // d_res[0] = <s, t>
     B2K_TRY(b2k_enqueue_dot(ctx, rt.ptr, rt.ptr, n, nullptr, -1, 1, -1));       // d_res[1] = <t, t>
     B2K_TRY(b2k_allreduce(ctx, ctx->d_res, 2, rr.sharded));
     const int grid = grid_for(ctx, n, 8);
-    if (ctx->dtype == B2K_F64)
-        k_bicg_xr<double><<<grid, BT, 0, ctx->stream>>>((double*)rx.ptr, (double*)rr.ptr, (const double*)rrs.ptr,
-                                                        (const double*)rp.ptr, (const double*)rsv.ptr,
-                                                        (const double*)rt.ptr, n, alpha, ctx->d_res,
-                                                        ctx->d_res + 1, ctx->d_part_s, ctx->d_sync,
-                                                        ctx->d_res + 2, BicgChain{});
-    else
-        k_bicg_xr<float><<<grid, BT, 0, ctx->stream>>>((float*)rx.ptr, (float*)rr.ptr, (const float*)rrs.ptr,
-                                                       (const float*)rp.ptr, (const float*)rsv.ptr,
-                                                       (const float*)rt.ptr, n, (float)alpha, ctx->d_res,
-                                                       ctx->d_res + 1, ctx->d_part_s, ctx->d_sync,
-                                                       ctx->d_res + 2, BicgChain{});
+    b2k_dispatch(ctx, [&](auto tt) {
+        using T = decltype(tt);
+        k_bicg_xr<T><<<grid, BT, 0, ctx->stream>>>((T*)rx.ptr, (T*)rr.ptr, (const T*)rrs.ptr, (const T*)rp.ptr,
+                                                   (const T*)rsv.ptr, (const T*)rt.ptr, n, T(alpha), ctx->d_res,
+                                                   ctx->d_res + 1, ctx->d_part_s, ctx->d_sync, ctx->d_res + 2,
+                                                   BicgChain{});
+    });
     B2K_LAUNCH_CHECK(ctx);
     B2K_TRY(b2k_allreduce(ctx, ctx->d_res + 2, 2, rr.sharded));
     B2K_TRY(b2k_fetch_results(ctx, 4, 0));
@@ -1526,80 +1449,56 @@ extern "C" int32_t b2k_bicgstab_chain(b2k_ctx* ctx, const b2k_op* op, b2k_vec x,
     if (!ctx || !op || !rec_out || !steps_done || nsteps < 1) return B2K_EINVAL;
     *steps_done = 0;
     if (nsteps > B2K_MAX_CHAIN - 1) nsteps = B2K_MAX_CHAIN - 1;
-    VecRef rx, rr, rrs, rp, rv, rsv, rt;
-    B2K_TRY(b2k_resolve(ctx, x, &rx));
-    B2K_TRY(b2k_resolve(ctx, r, &rr));
-    B2K_TRY(b2k_resolve(ctx, rs, &rrs));
-    B2K_TRY(b2k_resolve(ctx, p, &rp));
-    B2K_TRY(b2k_resolve(ctx, v, &rv));
-    B2K_TRY(b2k_resolve(ctx, s, &rsv));
-    B2K_TRY(b2k_resolve(ctx, t, &rt));
+    VecRef vr[7];
+    B2K_TRY(b2k_resolve_vecs(ctx, "bicgstab_chain", {x, r, rs, p, v, s, t}, vr, true));
+    const VecRef &rx = vr[0], &rr = vr[1], &rrs = vr[2], &rp = vr[3], &rv = vr[4], &rsv = vr[5], &rt = vr[6];
     const int64_t n = rr.n;
-    if (rx.n != n || rrs.n != n || rp.n != n || rv.n != n || rsv.n != n || rt.n != n)
-        return b2k_fail(ctx, B2K_EDIM, "bicgstab_chain: length mismatch");
     if (ctx->nranks > 1)
         return b2k_fail(ctx, B2K_ENOTSUP, "bicgstab_chain: single-GPU contexts (use b2k_bicgstab_half/_full)");
     int64_t orows = 0, ocols = 0;
     int32_t okind = -1;
     B2K_TRY(b2k_op_info(op, &orows, &ocols, nullptr, &okind));
     if (okind != 0) return b2k_fail(ctx, B2K_ENOTSUP, "bicgstab_chain: CSR operators only");
-    double* st = ctx->d_steps;                          // {rho, rho_old, alpha, omega}
-    double* rec0 = ctx->d_steps + B2K_REC;
-    int* d_stop = reinterpret_cast<int*>(ctx->d_sync + B2K_SYNC_STOP);
+    B2kChain fr(ctx, B2K_REC);                          // state {rho, rho_old, alpha, omega}
     const double seed[4] = {rho, rho_old, alpha, omega};
-    B2K_TRY(b2k_put_coef(ctx, seed, 4, 0));
-    B2K_CUDA(ctx, cudaMemcpyAsync(st, ctx->d_coef, 4 * sizeof(double), cudaMemcpyDeviceToDevice, ctx->stream));
-    B2K_CUDA(ctx, cudaMemsetAsync(rec0, 0, sizeof(double) * B2K_REC * nsteps, ctx->stream));
-    B2K_CUDA(ctx, cudaMemsetAsync(d_stop, 0, sizeof(int), ctx->stream));
+    B2K_TRY(fr.seed(seed, 4, nsteps));
     const bool shifted = (a0 != 0.0) || (a1 != 1.0);
     const int grid = grid_for(ctx, n, 8);
-    const bool f64 = ctx->dtype == B2K_F64;
     SpmvFuse fz;
     memset(&fz, 0, sizeof(fz));
-    fz.stop = d_stop;
-    for (int32_t i = 0; i < nsteps; ++i) {
-        BicgChain ch;
-        ch.st = st; ch.rec = rec0 + (size_t)B2K_REC * i; ch.stop = d_stop; ch.tol = tol;
-        if (f64)
-            k_bicg_p<double><<<grid, BT, 0, ctx->stream>>>((double*)rp.ptr, (const double*)rr.ptr,
-                                                           (const double*)rv.ptr, n, 0.0, 0.0, ch);
-        else
-            k_bicg_p<float><<<grid, BT, 0, ctx->stream>>>((float*)rp.ptr, (const float*)rr.ptr,
-                                                          (const float*)rv.ptr, n, 0.f, 0.f, ch);
-        B2K_LAUNCH_CHECK(ctx);
-        B2K_TRY(b2k_enqueue_apply_fused(ctx, op, rp, rv, a0, a1, shifted, &rrs, ctx->d_res, &fz));   // sigma
-        if (f64)
-            k_bicg_s<double><<<grid, BT, 0, ctx->stream>>>((double*)rsv.ptr, (const double*)rr.ptr,
-                                                           (const double*)rv.ptr, n, 0.0, ctx->d_res, ctx->d_part_s,
-                                                           ctx->d_sync, ctx->d_res + 1, ch);
-        else
-            k_bicg_s<float><<<grid, BT, 0, ctx->stream>>>((float*)rsv.ptr, (const float*)rr.ptr,
-                                                          (const float*)rv.ptr, n, 0.0, ctx->d_res, ctx->d_part_s,
-                                                          ctx->d_sync, ctx->d_res + 1, ch);
-        B2K_LAUNCH_CHECK(ctx);
-        B2K_TRY(b2k_enqueue_apply_fused(ctx, op, rsv, rt, a0, a1, shifted, &rsv, ctx->d_res, &fz));  // <s, t>
-        B2K_TRY(b2k_enqueue_dot(ctx, rt.ptr, rt.ptr, n, nullptr, -1, 1, -1));                        // <t, t>
-        if (f64)
-            k_bicg_xr<double><<<grid, BT, 0, ctx->stream>>>((double*)rx.ptr, (double*)rr.ptr, (const double*)rrs.ptr,
-                                                            (const double*)rp.ptr, (const double*)rsv.ptr,
-                                                            (const double*)rt.ptr, n, 0.0, ctx->d_res,
-                                                            ctx->d_res + 1, ctx->d_part_s, ctx->d_sync,
-                                                            ctx->d_res + 2, ch);
-        else
-            k_bicg_xr<float><<<grid, BT, 0, ctx->stream>>>((float*)rx.ptr, (float*)rr.ptr, (const float*)rrs.ptr,
-                                                           (const float*)rp.ptr, (const float*)rsv.ptr,
-                                                           (const float*)rt.ptr, n, 0.f, ctx->d_res,
-                                                           ctx->d_res + 1, ctx->d_part_s, ctx->d_sync,
-                                                           ctx->d_res + 2, ch);
-        B2K_LAUNCH_CHECK(ctx);
-    }
-    B2K_CUDA(ctx, cudaMemcpyAsync(ctx->h_res, rec0, sizeof(double) * B2K_REC * nsteps, cudaMemcpyDeviceToHost,
-                                  ctx->stream));
-    B2K_TRY(b2k_stream_sync(ctx));
-    int32_t d = nsteps;
-    for (int32_t i = 0; i < nsteps; ++i)
-        if (ctx->h_res[(size_t)B2K_REC * i + 7] != 0.0) { d = i + 1; break; }
-    memcpy(rec_out, ctx->h_res, sizeof(double) * B2K_REC * d);
+    fz.stop = fr.stop;
+    B2K_TRY(fr.enqueue([&]() -> int32_t {
+        for (int32_t i = 0; i < nsteps; ++i) {
+            const BicgChain ch{fr.st, fr.rec0 + (size_t)B2K_REC * i, fr.stop, tol};
+            b2k_dispatch(ctx, [&](auto tt) {
+                using T = decltype(tt);
+                k_bicg_p<T><<<grid, BT, 0, ctx->stream>>>((T*)rp.ptr, (const T*)rr.ptr, (const T*)rv.ptr, n, T(0),
+                                                          T(0), ch);
+            });
+            B2K_LAUNCH_CHECK(ctx);
+            B2K_TRY(b2k_enqueue_apply_fused(ctx, op, rp, rv, a0, a1, shifted, &rrs, ctx->d_res, &fz));   // sigma
+            b2k_dispatch(ctx, [&](auto tt) {
+                using T = decltype(tt);
+                k_bicg_s<T><<<grid, BT, 0, ctx->stream>>>((T*)rsv.ptr, (const T*)rr.ptr, (const T*)rv.ptr, n, 0.0,
+                                                          ctx->d_res, ctx->d_part_s, ctx->d_sync, ctx->d_res + 1, ch);
+            });
+            B2K_LAUNCH_CHECK(ctx);
+            B2K_TRY(b2k_enqueue_apply_fused(ctx, op, rsv, rt, a0, a1, shifted, &rsv, ctx->d_res, &fz));  // <s, t>
+            B2K_TRY(b2k_enqueue_dot(ctx, rt.ptr, rt.ptr, n, nullptr, -1, 1, -1));                        // <t, t>
+            b2k_dispatch(ctx, [&](auto tt) {
+                using T = decltype(tt);
+                k_bicg_xr<T><<<grid, BT, 0, ctx->stream>>>((T*)rx.ptr, (T*)rr.ptr, (const T*)rrs.ptr, (const T*)rp.ptr,
+                                                           (const T*)rsv.ptr, (const T*)rt.ptr, n, T(0), ctx->d_res,
+                                                           ctx->d_res + 1, ctx->d_part_s, ctx->d_sync, ctx->d_res + 2,
+                                                           ch);
+            });
+            B2K_LAUNCH_CHECK(ctx);
+        }
+        return B2K_OK;
+    }));
+    B2K_TRY(fr.fetch(nsteps));
+    const int32_t d = fr.count(nsteps, [](const double* rec) { return rec[7] != 0.0; });
+    memcpy(rec_out, fr.hrec, sizeof(double) * B2K_REC * d);
     *steps_done = d;
     return B2K_OK;
 }
@@ -1612,69 +1511,53 @@ extern "C" int32_t b2k_minres_chain(b2k_ctx* ctx, const b2k_op* op, b2k_vec x, b
                                     int32_t nsteps, double* rec_out, double* state_out, int32_t* steps_done) {
     if (!ctx || !op || !state_in || !rec_out || !state_out || !steps_done || nsteps < 1) return B2K_EINVAL;
     if (nsteps > B2K_MAX_CHAIN - 1) nsteps = B2K_MAX_CHAIN - 1;
-    const b2k_vec hv[6] = {x, p_prev, p_cur, q, d1, d2};
     VecRef r[6];
-    for (int i = 0; i < 6; ++i) B2K_TRY(b2k_resolve(ctx, hv[i], &r[i]));
+    B2K_TRY(b2k_resolve_vecs(ctx, "minres_chain", {x, p_prev, p_cur, q, d1, d2}, r, true));
     const int64_t n = r[0].n;
     int64_t orows = 0, ocols = 0;
     int32_t okind = -1;
     B2K_TRY(b2k_op_info(op, &orows, &ocols, nullptr, &okind));
     if (ctx->nranks > 1) return b2k_fail(ctx, B2K_ENOTSUP, "minres_chain: single-GPU contexts only");
     if (okind == 1) return b2k_fail(ctx, B2K_ENOTSUP, "minres_chain: CSR / stencil operators only");
-    for (int i = 0; i < 6; ++i)
-        if (r[i].n != n || orows != n || ocols != n) return b2k_fail(ctx, B2K_EDIM, "minres_chain: length mismatch");
-    for (int i = 0; i < 6; ++i)
-        for (int j = 0; j < i; ++j)
-            if (r[i].ptr == r[j].ptr) return b2k_fail(ctx, B2K_EINVAL, "minres_chain: vectors %d and %d are the same", j, i);
+    if (orows != n || ocols != n) return b2k_fail(ctx, B2K_EDIM, "minres_chain: length mismatch");
     *steps_done = 0;
-    double* st = ctx->d_steps;
-    double* rec0 = ctx->d_steps + MR_NSTATE;
-    int* d_stop = reinterpret_cast<int*>(ctx->d_sync + B2K_SYNC_STOP);
+    B2kChain fr(ctx, MR_NSTATE);
     double seed[MR_NSTATE] = {};
     memcpy(seed, state_in, 8 * sizeof(double));
-    B2K_TRY(b2k_put_coef(ctx, seed, MR_NSTATE, 0));
-    B2K_CUDA(ctx, cudaMemcpyAsync(st, ctx->d_coef, MR_NSTATE * sizeof(double), cudaMemcpyDeviceToDevice, ctx->stream));
-    B2K_CUDA(ctx, cudaMemsetAsync(rec0, 0, sizeof(double) * B2K_REC * nsteps, ctx->stream));
-    B2K_CUDA(ctx, cudaMemsetAsync(d_stop, 0, sizeof(int), ctx->stream));
+    B2K_TRY(fr.seed(seed, MR_NSTATE, nsteps));
     const bool shifted = (a0 != 0.0) || (a1 != 1.0);
     const int grid = grid_for(ctx, n, 4);
-    const bool f64 = ctx->dtype == B2K_F64;
     SpmvFuse fz;
     memset(&fz, 0, sizeof(fz));
-    fz.stop = d_stop;
-    fz.xscale = st + MR_INVB;
+    fz.stop = fr.stop;
+    fz.xscale = fr.st + MR_INVB;
     fz.dot_self = 1;
     MinresChain ch;
-    ch.st = st; ch.stop = d_stop; ch.alpha = ctx->d_res; ch.tol = tol;
-#define LAUNCH(T, LZ)                                                                                       \
-    k_minres_step<T, LZ><<<grid, BT, 0, ctx->stream>>>((T*)r[0].ptr, (T*)r[1].ptr, (T*)r[2].ptr,            \
-                                                       (const T*)r[3].ptr, (T*)r[4].ptr, (T*)r[5].ptr, n,   \
-                                                       ctx->d_part_s, ctx->d_sync, ch)
-    for (int32_t i = 0; i <= nsteps; ++i) {
-        ch.rec = rec0 + (size_t)B2K_REC * i;
-        if (i == nsteps) {                         // flush
-            if (f64) LAUNCH(double, false);
-            else LAUNCH(float, false);
-        } else {
+    ch.st = fr.st; ch.stop = fr.stop; ch.alpha = ctx->d_res; ch.tol = tol;
+    B2K_TRY(fr.enqueue([&]() -> int32_t {
+        for (int32_t i = 0; i <= nsteps; ++i) {
+            ch.rec = fr.rec0 + (size_t)B2K_REC * i;
             // the operand is p_cur of this iteration: the roles swap with every iteration that runs, and a launch
             // behind a raised stop flag does nothing, so the host's count is the device's whenever it matters
-            B2K_TRY(b2k_enqueue_apply_fused(ctx, op, r[(i & 1) ? 1 : 2], r[3], a0, a1, shifted, nullptr, ctx->d_res, &fz));
-            if (f64) LAUNCH(double, true);
-            else LAUNCH(float, true);
+            if (i < nsteps)
+                B2K_TRY(b2k_enqueue_apply_fused(ctx, op, r[(i & 1) ? 1 : 2], r[3], a0, a1, shifted, nullptr, ctx->d_res,
+                                                &fz));
+            b2k_dispatch(ctx, [&](auto t) {
+                using T = decltype(t);
+                b2k_flag(i < nsteps, [&](auto lz) {            // the last launch is the flush
+                    k_minres_step<T, lz><<<grid, BT, 0, ctx->stream>>>((T*)r[0].ptr, (T*)r[1].ptr, (T*)r[2].ptr,
+                                                                       (const T*)r[3].ptr, (T*)r[4].ptr, (T*)r[5].ptr,
+                                                                       n, ctx->d_part_s, ctx->d_sync, ch);
+                });
+            });
+            B2K_LAUNCH_CHECK(ctx);
         }
-        B2K_LAUNCH_CHECK(ctx);
-    }
-#undef LAUNCH
-    // state and records are one block of d_steps
-    B2K_CUDA(ctx, cudaMemcpyAsync(ctx->h_res, st, sizeof(double) * (MR_NSTATE + B2K_REC * nsteps), cudaMemcpyDeviceToHost,
-                                  ctx->stream));
-    B2K_TRY(b2k_stream_sync(ctx));
-    const double* hrec = ctx->h_res + MR_NSTATE;
-    int32_t d = nsteps;
-    for (int32_t i = 0; i < nsteps; ++i)
-        if (hrec[(size_t)B2K_REC * i + 5] != 0.0) { d = i + 1; break; }
-    memcpy(rec_out, hrec, sizeof(double) * B2K_REC * d);
-    memcpy(state_out, ctx->h_res, 8 * sizeof(double));
+        return B2K_OK;
+    }));
+    B2K_TRY(fr.fetch(nsteps, 8));
+    const int32_t d = fr.count(nsteps, [](const double* rec) { return rec[5] != 0.0; });
+    memcpy(rec_out, fr.hrec, sizeof(double) * B2K_REC * d);
+    memcpy(state_out, fr.hst, 8 * sizeof(double));
     *steps_done = d;
     return B2K_OK;
 }

@@ -519,8 +519,7 @@ int32_t block_project_dev(b2k_ctx* ctx, const BPanel& bp, double* d_H, bool accu
     const int k = (int)bp.q.size(), p = (int)bp.r.size();
     for (int q0 = 0; q0 < k; q0 += BK_QMAX) {
         const int kq = std::min(BK_QMAX, k - q0);
-        if (ctx->dtype == B2K_F64) B2K_TRY(launch_project<double>(ctx, bp, q0, kq, d_H, k, accumulate));
-        else B2K_TRY(launch_project<float>(ctx, bp, q0, kq, d_H, k, accumulate));
+        B2K_TRY(b2k_dispatch(ctx, [&](auto t) { return launch_project<decltype(t)>(ctx, bp, q0, kq, d_H, k, accumulate); }));
     }
     if (!accumulate) B2K_TRY(b2k_allreduce(ctx, d_H, k * p, bp.sharded));
     return B2K_OK;
@@ -532,8 +531,7 @@ int32_t block_update_dev(b2k_ctx* ctx, const BPanel& bp, const double* d_H, doub
     for (int q0 = 0; q0 < k; q0 += BK_QMAX) {
         const int kq = std::min(BK_QMAX, k - q0);
         const bool lastp = q0 + kq >= k;
-        if (ctx->dtype == B2K_F64) B2K_TRY(launch_update<double>(ctx, bp, q0, kq, d_H, k, alpha, lastp ? d_G : nullptr, true));
-        else B2K_TRY(launch_update<float>(ctx, bp, q0, kq, d_H, k, alpha, lastp ? d_G : nullptr, true));
+        B2K_TRY(b2k_dispatch(ctx, [&](auto t) { return launch_update<decltype(t)>(ctx, bp, q0, kq, d_H, k, alpha, lastp ? d_G : nullptr, true); }));
     }
     if (d_G) B2K_TRY(b2k_allreduce(ctx, d_G, p * p, bp.sharded));
     return B2K_OK;
@@ -550,16 +548,16 @@ int32_t block_rmul_upper(b2k_ctx* ctx, const BPanel& bp, const double* U, double
     rp.gpart = d_G ? ctx->d_blkpart : nullptr;
     const int grid = (int)std::max<int64_t>(1, std::min<int64_t>((bp.n + 511) / 512, 4 * (int64_t)ctx->num_sms));
     const int pr = b2k_prof_begin(ctx, 6, 2.0 * p * ctx->esize * (double)bp.n);
-#define RMUL(T, P) k_block_rmul<T, P><<<grid, 256, 0, ctx->stream>>>(rp)
-#define RMUL_P(T)                                                                                      \
-    switch (p) {                                                                                       \
-        case 1: RMUL(T, 1); break; case 2: RMUL(T, 2); break; case 3: RMUL(T, 3); break;               \
-        case 4: RMUL(T, 4); break; case 5: RMUL(T, 5); break; case 6: RMUL(T, 6); break;               \
-        case 7: RMUL(T, 7); break; default: RMUL(T, 8); break;                                         \
-    }
-    if (ctx->dtype == B2K_F64) { RMUL_P(double) } else { RMUL_P(float) }
-#undef RMUL_P
+    b2k_dispatch(ctx, [&](auto t) {
+        using T = decltype(t);
+#define RMUL(P) k_block_rmul<T, P><<<grid, 256, 0, ctx->stream>>>(rp)
+        switch (p) {
+            case 1: RMUL(1); break; case 2: RMUL(2); break; case 3: RMUL(3); break;
+            case 4: RMUL(4); break; case 5: RMUL(5); break; case 6: RMUL(6); break;
+            case 7: RMUL(7); break; default: RMUL(8); break;
+        }
 #undef RMUL
+    });
     b2k_prof_end(ctx, pr);
     B2K_LAUNCH_CHECK(ctx);
     if (d_G) {
@@ -572,8 +570,7 @@ int32_t block_rmul_upper(b2k_ctx* ctx, const BPanel& bp, const double* U, double
 
 int32_t block_gram_dev(b2k_ctx* ctx, const BPanel& bp, double* d_G) {
     const int p = (int)bp.r.size();
-    if (ctx->dtype == B2K_F64) B2K_TRY(launch_update<double>(ctx, bp, 0, 0, nullptr, 1, 0.0, d_G, false));
-    else B2K_TRY(launch_update<float>(ctx, bp, 0, 0, nullptr, 1, 0.0, d_G, false));
+    B2K_TRY(b2k_dispatch(ctx, [&](auto t) { return launch_update<decltype(t)>(ctx, bp, 0, 0, nullptr, 1, 0.0, d_G, false); }));
     return b2k_allreduce(ctx, d_G, p * p, bp.sharded);
 }
 
@@ -677,8 +674,7 @@ extern "C" int32_t b2k_block_orthogonalize(b2k_ctx* ctx, const b2k_vec* Rb, int3
     B2K_TRY(block_project_dev(ctx, bp, d_H1, false));
     if (passes == 2 && p <= 4 && k <= BK_QMAX && g_block_fuse) {
         // three sweeps over V: project | update + project of the updated block on the resident tile | update (+ Gram)
-        if (ctx->dtype == B2K_F64) B2K_TRY(launch_update_project<double>(ctx, bp, d_H1, -1.0, d_H2));
-        else B2K_TRY(launch_update_project<float>(ctx, bp, d_H1, -1.0, d_H2));
+        B2K_TRY(b2k_dispatch(ctx, [&](auto t) { return launch_update_project<decltype(t)>(ctx, bp, d_H1, -1.0, d_H2); }));
         B2K_TRY(block_update_dev(ctx, bp, d_H2, -1.0, G_host ? d_G : nullptr));
     } else {
         B2K_TRY(block_update_dev(ctx, bp, d_H1, -1.0, (passes == 1 && G_host) ? d_G : nullptr));

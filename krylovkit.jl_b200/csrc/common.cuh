@@ -5,7 +5,9 @@
 #include <cstdint>
 #include <cstdio>
 #include <cstring>
+#include <initializer_list>
 #include <string>
+#include <type_traits>
 #include <vector>
 #include "../../include/b200krylov.h"
 
@@ -136,6 +138,27 @@ int32_t b2k_resolve(b2k_ctx* ctx, b2k_vec v, VecRef* out);
 // all handles must share one space; fills col indices; returns space id in *space
 int32_t b2k_resolve_cols(b2k_ctx* ctx, const b2k_vec* cols, int32_t k, int32_t* space,
                          std::vector<int32_t>* idx);
+// The vector arguments of an entry point: resolves the handles into out[0 .. hs.size()), which must all have one
+// length (B2K_EDIM, "<entry>: length mismatch") and, with distinct, be pairwise different vectors (B2K_EINVAL,
+// "<entry>: vectors j and i are the same").
+int32_t b2k_resolve_vecs(b2k_ctx* ctx, const char* entry, std::initializer_list<b2k_vec> hs, VecRef* out,
+                         bool distinct = false);
+
+// Calls f(T()) with T the vector type of the context (double or float): one launch statement serves both instances.
+template <typename F>
+inline decltype(auto) b2k_dispatch(const b2k_ctx* ctx, F&& f) {
+    if (ctx->dtype == B2K_F64) return f(double());
+    return f(float());
+}
+// Calls f(std::true_type()) or f(std::false_type()): a run-time flag picks one of two template instances.
+template <typename F>
+inline decltype(auto) b2k_flag(bool b, F&& f) {
+    if (b) return f(std::true_type());
+    return f(std::false_type());
+}
+
+// eps(T) of the context's vector type (the tolerance floor of the iterative-refinement loops, orthonormal.jl:481)
+inline double b2k_eps(const b2k_ctx* ctx) { return ctx->dtype == B2K_F64 ? 0x1p-52 : 0x1p-23; }
 
 // scalar plumbing (ctx.cu)
 // reduce-across-ranks (if sharded & dist) the first `count` doubles of d_res, copy to h_res, sync.
@@ -144,6 +167,58 @@ int32_t b2k_fetch_results(b2k_ctx* ctx, int32_t count, int32_t sharded);
 int32_t b2k_allreduce(b2k_ctx* ctx, double* dptr, int32_t count, int32_t sharded);
 // upload `count` doubles of host coefficients into d_coef + offset (async, pinned staging)
 int32_t b2k_put_coef(b2k_ctx* ctx, const double* host, int32_t count, int32_t offset);
+
+// The step records of a call that chains its iterations on the device (CG, BiCGStab, MINRES, LSMR, Lanczos, GKL):
+// a state block of nstate doubles at d_steps, then rec_len doubles per iteration, and the stop flag the recurrence
+// raises (every later launch of the call then does nothing); LSMR adds the skip flag of its A' side.
+// Once anything is enqueued, an error return goes through fail(): the launches already queued write the caller's
+// vectors, so the call waits for them before it returns.
+struct B2kChain {
+    b2k_ctx* ctx;
+    double* st;
+    double* rec0;
+    int* stop;
+    int* skip;
+    int nstate, rec_len;
+    const double* hrec = nullptr;   // fetch(): the records on the host
+    const double* hst = nullptr;    // fetch(nrec, nst): the first nst doubles of the state on the host
+
+    B2kChain(b2k_ctx* ctx, int nstate, int rec_len = B2K_REC);
+    // state <- s[0, ns) through the coefficient staging, stop flag (and skip flag) <- 0, records [0, nclear) <- 0
+    int32_t seed(const double* s, int ns, int nclear, bool with_skip = false);
+    // runs the enqueueing function f; an error from it is returned after the stream has drained
+    template <typename F> int32_t enqueue(F&& f) {
+        const int32_t rc = f();
+        return rc == B2K_OK ? rc : fail(rc);
+    }
+    int32_t fail(int32_t rc);
+    // copies records [0, nrec) (and the first nst doubles of the state) to the host and synchronises
+    int32_t fetch(int nrec, int nst = 0);
+    // number of records up to and including the first one for which stops(rec) holds (nrec if none does)
+    template <typename F> int32_t count(int nrec, F&& stops) const {
+        for (int i = 0; i < nrec; ++i)
+            if (stops(hrec + (size_t)rec_len * i)) return i + 1;
+        return nrec;
+    }
+};
+
+// Column bookkeeping of a chained Lanczos or GKL batch.  Each step allocates its columns; at the end every column the
+// batch touched is free again except those of the d steps that ran (later steps were skipped on the device, and
+// steps enqueued before an error are kept too): step i leaves its new basis vector in ucols[k + i] (and GKL's v in
+// vcols[k + i]), the last one its residual in ucols[k + d].  Nothing ran: the residual handed in stays.
+struct B2kChainCols {
+    b2k_ctx* ctx;
+    std::vector<b2k_vec> touched, u, v, w;
+
+    B2kChainCols(b2k_ctx* ctx, b2k_vec r) : ctx(ctx), touched{r} {}
+    int32_t alloc(int32_t space, b2k_vec* h);
+    // the column of h has been read for the last time: later steps may reuse it (stream order keeps that safe)
+    void consumed(b2k_vec h);
+    // step of the batch enqueued: its new basis vector(s) (vi = -1 for Lanczos) and residual
+    void ran(b2k_vec ui, b2k_vec vi, b2k_vec wi);
+    // keeps the d steps that ran; returns the residual that follows them
+    b2k_vec commit(int32_t d, b2k_vec* ucols, b2k_vec* vcols, int32_t k);
+};
 
 // Device memory comes from the CUDA stream-ordered pool with an unbounded release
 // threshold: a cudaMalloc/cudaFree of a multi-GB slab per solve would dominate the

@@ -386,6 +386,21 @@ int32_t b2k_resolve_cols(b2k_ctx* ctx, const b2k_vec* cols, int32_t k, int32_t* 
     return B2K_OK;
 }
 
+int32_t b2k_resolve_vecs(b2k_ctx* ctx, const char* entry, std::initializer_list<b2k_vec> hs, VecRef* out,
+                         bool distinct) {
+    const int n = (int)hs.size();
+    int i = 0;
+    for (b2k_vec h : hs) B2K_TRY(b2k_resolve(ctx, h, &out[i++]));
+    for (i = 1; i < n; ++i)
+        if (out[i].n != out[0].n) return b2k_fail(ctx, B2K_EDIM, "%s: length mismatch", entry);
+    if (distinct)
+        for (i = 0; i < n; ++i)
+            for (int j = 0; j < i; ++j)
+                if (out[i].ptr == out[j].ptr)
+                    return b2k_fail(ctx, B2K_EINVAL, "%s: vectors %d and %d are the same", entry, j, i);
+    return B2K_OK;
+}
+
 extern "C" int32_t b2k_vec_alloc(b2k_ctx* ctx, int32_t space, b2k_vec* out) {
     if (!ctx || !out) return B2K_EINVAL;
     if (space < 0 || space >= (int32_t)ctx->spaces.size())
@@ -516,6 +531,79 @@ int32_t b2k_put_coef(b2k_ctx* ctx, const double* host, int32_t count, int32_t of
     B2K_CUDA(ctx, cudaEventRecord(ctx->ev_coef, ctx->stream));
     ctx->coef_busy = true;
     return B2K_OK;
+}
+
+// ------------------------------------------------------------ chained calls ----
+
+B2kChain::B2kChain(b2k_ctx* c, int ns, int rl)
+    : ctx(c), st(c->d_steps), rec0(c->d_steps + ns), stop(reinterpret_cast<int*>(c->d_sync + B2K_SYNC_STOP)),
+      skip(reinterpret_cast<int*>(c->d_sync + B2K_SYNC_SKIP)), nstate(ns), rec_len(rl) {}
+
+int32_t B2kChain::seed(const double* s, int ns, int nclear, bool with_skip) {
+    return enqueue([&]() -> int32_t {
+        B2K_TRY(b2k_put_coef(ctx, s, ns, 0));
+        B2K_CUDA(ctx, cudaMemcpyAsync(st, ctx->d_coef, ns * sizeof(double), cudaMemcpyDeviceToDevice, ctx->stream));
+        if (nclear > 0)
+            B2K_CUDA(ctx, cudaMemsetAsync(rec0, 0, sizeof(double) * rec_len * nclear, ctx->stream));
+        B2K_CUDA(ctx, cudaMemsetAsync(stop, 0, sizeof(int), ctx->stream));
+        if (with_skip) B2K_CUDA(ctx, cudaMemsetAsync(skip, 0, sizeof(int), ctx->stream));
+        return B2K_OK;
+    });
+}
+
+int32_t B2kChain::fail(int32_t rc) {
+    cudaStreamSynchronize(ctx->stream);
+    return rc;
+}
+
+int32_t B2kChain::fetch(int nrec, int nst) {
+    const size_t rbytes = sizeof(double) * rec_len * nrec;
+    B2K_TRY(enqueue([&]() -> int32_t {
+        if (nst > 0 && nstate + (size_t)rec_len * nrec <= (size_t)B2K_RES_DOUBLES) {
+            // state and records are one block of d_steps
+            hst = ctx->h_res;
+            hrec = ctx->h_res + nstate;
+            B2K_CUDA(ctx, cudaMemcpyAsync(ctx->h_res, st, sizeof(double) * nstate + rbytes, cudaMemcpyDeviceToHost,
+                                          ctx->stream));
+            return B2K_OK;
+        }
+        hrec = ctx->h_res;
+        hst = ctx->h_res + B2K_RES_DOUBLES - nst;
+        B2K_CUDA(ctx, cudaMemcpyAsync(ctx->h_res, rec0, rbytes, cudaMemcpyDeviceToHost, ctx->stream));
+        if (nst > 0)
+            B2K_CUDA(ctx, cudaMemcpyAsync(ctx->h_res + B2K_RES_DOUBLES - nst, st, sizeof(double) * nst,
+                                          cudaMemcpyDeviceToHost, ctx->stream));
+        return B2K_OK;
+    }));
+    return b2k_stream_sync(ctx);
+}
+
+int32_t B2kChainCols::alloc(int32_t space, b2k_vec* h) {
+    B2K_TRY(b2k_vec_alloc(ctx, space, h));
+    touched.push_back(*h);
+    return B2K_OK;
+}
+
+void B2kChainCols::consumed(b2k_vec h) { ctx->spaces[B2K_VEC_SPACE(h)].used[B2K_VEC_COL(h)] = 0; }
+
+void B2kChainCols::ran(b2k_vec ui, b2k_vec vi, b2k_vec wi) {
+    u.push_back(ui);
+    v.push_back(vi);
+    w.push_back(wi);
+}
+
+b2k_vec B2kChainCols::commit(int32_t d, b2k_vec* ucols, b2k_vec* vcols, int32_t k) {
+    auto keep = [&](b2k_vec* cols, int32_t i, b2k_vec h) {
+        cols[i] = h;
+        ctx->spaces[B2K_VEC_SPACE(h)].used[B2K_VEC_COL(h)] = 1;
+    };
+    for (b2k_vec h : touched) consumed(h);
+    for (int32_t i = 0; i < d; ++i) {          // (skipped steps overwrote the columns behind ucols[k + d])
+        keep(ucols, k + i, u[i]);
+        if (vcols) keep(vcols, k + i, v[i]);
+    }
+    keep(ucols, k + d, d > 0 ? w[d - 1] : touched[0]);
+    return ucols[k + d];
 }
 
 // ------------------------------------------------------------------ profiling ----

@@ -1719,12 +1719,10 @@ extern "C" int32_t b2k_op_create_stencil(b2k_ctx* ctx, b2k_op** out, int64_t nx,
     CK(B2K_DMALLOC(&op->vals, (size_t)ctx->esize * (std::max<int64_t>(1, op->nnz) + 8)));
     CK(B2K_DMALLOC(&d_gcol, sizeof(int64_t) * std::max<int64_t>(1, op->nnz)));
     if (n_loc > 0) {
-        if (ctx->dtype == B2K_F64)
-            k_stencil_fill<double><<<blocks, 256, 0, ctx->stream>>>(d, op->rowptr, d_gcol,
-                                                                    (double*)op->vals);
-        else
-            k_stencil_fill<float><<<blocks, 256, 0, ctx->stream>>>(d, op->rowptr, d_gcol,
-                                                                   (float*)op->vals);
+        b2k_dispatch(ctx, [&](auto t) {
+            using T = decltype(t);
+            k_stencil_fill<T><<<blocks, 256, 0, ctx->stream>>>(d, op->rowptr, d_gcol, (T*)op->vals);
+        });
         ctx->launches++;
     }
 #undef CK
@@ -1836,12 +1834,11 @@ extern "C" int32_t b2k_op_create_dense_splitmix(b2k_ctx* ctx, b2k_op** out, int6
     B2K_TRY(alloc_dense(ctx, out, m_local, n));
     b2k_op* op = *out;
     const uint64_t mg = ctx->nranks > 1 ? (uint64_t)ctx->n_global : (uint64_t)m_local;
-    if (ctx->dtype == B2K_F64)
-        k_dense_fill_splitmix<double><<<ctx->num_sms * 8, 256, 0, ctx->stream>>>(
-            (double*)op->A, m_local, n, op->ld, seed, (uint64_t)ctx->row_offset, mg);
-    else
-        k_dense_fill_splitmix<float><<<ctx->num_sms * 8, 256, 0, ctx->stream>>>(
-            (float*)op->A, m_local, n, op->ld, seed, (uint64_t)ctx->row_offset, mg);
+    b2k_dispatch(ctx, [&](auto t) {
+        using T = decltype(t);
+        k_dense_fill_splitmix<T><<<ctx->num_sms * 8, 256, 0, ctx->stream>>>((T*)op->A, m_local, n, op->ld, seed,
+                                                                            (uint64_t)ctx->row_offset, mg);
+    });
     B2K_LAUNCH_CHECK(ctx);
     return B2K_OK;
 }
@@ -2006,12 +2003,11 @@ extern "C" int32_t b2k_op_create_transpose(b2k_ctx* ctx, b2k_op** out, const b2k
         CK(B2K_DMALLOC(&tmp, tmp_bytes));
         CK(cub::DeviceRadixSort::SortPairs(tmp, tmp_bytes, keys, scol, iota, perm, (int)nnz, 0, end_bit,
                                            ctx->stream));
-        if (ctx->dtype == B2K_F64)
-            k_transpose_gather<double><<<g, 256, 0, ctx->stream>>>(op->rowptr, n, (const double*)op->vals, perm, nnz,
-                                                                   t->colidx, (double*)t->vals);
-        else
-            k_transpose_gather<float><<<g, 256, 0, ctx->stream>>>(op->rowptr, n, (const float*)op->vals, perm, nnz,
-                                                                  t->colidx, (float*)t->vals);
+        b2k_dispatch(ctx, [&](auto tt) {
+            using T = decltype(tt);
+            k_transpose_gather<T><<<g, 256, 0, ctx->stream>>>(op->rowptr, n, (const T*)op->vals, perm, nnz, t->colidx,
+                                                              (T*)t->vals);
+        });
         ctx->launches++;
     }
     k_transpose_rowptr<<<g, 256, 0, ctx->stream>>>(scol, nnz, m, t->rowptr);
@@ -2254,12 +2250,11 @@ int32_t b2k_enqueue_apply_fused(b2k_ctx* ctx, const b2k_op* op, const VecRef& x,
                 const int64_t total = ps.send_lo + ps.send_hi;
                 if (total > 0) {
                     const int g = (int)std::max<int64_t>(1, std::min<int64_t>((total + 1023) / 1024, ctx->num_sms));
-                    if (ctx->dtype == B2K_F64)
-                        k_halo_push<double><<<g, 256, 0, ctx->stream>>>((const double*)x.ptr, x.n, ps,
-                                                                        ctx->d_sync + B2K_SYNC_HALO, fz.stop);
-                    else
-                        k_halo_push<float><<<g, 256, 0, ctx->stream>>>((const float*)x.ptr, x.n, ps,
-                                                                       ctx->d_sync + B2K_SYNC_HALO, fz.stop);
+                    b2k_dispatch(ctx, [&](auto t) {
+                        using T = decltype(t);
+                        k_halo_push<T><<<g, 256, 0, ctx->stream>>>((const T*)x.ptr, x.n, ps, ctx->d_sync + B2K_SYNC_HALO,
+                                                                   fz.stop);
+                    });
                     B2K_LAUNCH_CHECK(ctx);
                 }
             } else {
@@ -2297,15 +2292,12 @@ int32_t b2k_enqueue_apply_fused(b2k_ctx* ctx, const b2k_op* op, const VecRef& x,
         const int grid = (int)std::max<int64_t>(1, std::min<int64_t>((op->n_rows + 255) / 256, (int64_t)ctx->num_sms * 8));
         g_spmv_launch[0] = 4; g_spmv_launch[1] = 0; g_spmv_launch[2] = grid; g_spmv_launch[3] = 0;
         const int pr2 = b2k_prof_begin(ctx, 0, 2.0 * ctx->esize * op->n_rows);
-        if (ctx->dtype == B2K_F64)
-            k_stencil_apply<double><<<grid, 256, 0, ctx->stream>>>(sa, (const double*)xsrc, (const double*)halo, (double*)y.ptr,
-                                                                   a0, a1, shifted ? 1 : 0, dotv ? (const double*)dotv->ptr : nullptr,
-                                                                   op->part, ctx->d_sync, out, fz, ps);
-        else
-            k_stencil_apply<float><<<grid, 256, 0, ctx->stream>>>(sa, (const float*)xsrc, (const float*)halo, (float*)y.ptr,
-                                                                  (float)a0, (float)a1, shifted ? 1 : 0,
-                                                                  dotv ? (const float*)dotv->ptr : nullptr, op->part,
-                                                                  ctx->d_sync, out, fz, ps);
+        b2k_dispatch(ctx, [&](auto t) {
+            using T = decltype(t);
+            k_stencil_apply<T><<<grid, 256, 0, ctx->stream>>>(sa, (const T*)xsrc, (const T*)halo, (T*)y.ptr, T(a0), T(a1),
+                                                              shifted ? 1 : 0, dotv ? (const T*)dotv->ptr : nullptr,
+                                                              op->part, ctx->d_sync, out, fz, ps);
+        });
         b2k_prof_end(ctx, pr2);
         B2K_LAUNCH_CHECK(ctx);
         return B2K_OK;
@@ -2347,35 +2339,27 @@ int32_t b2k_enqueue_apply_fused(b2k_ctx* ctx, const b2k_op* op, const VecRef& x,
         const int per_sm = g_spmv_variant == 1 ? 4 : 3;
         const int grid = std::min(op->nblk, per_sm * ctx->num_sms);
         g_spmv_launch[0] = 2; g_spmv_launch[1] = g_spmv_variant; g_spmv_launch[2] = grid; g_spmv_launch[3] = op->nblk;
-#define LAUNCH_VG(T, NS, MB, GK)                                                               \
-    k_spmv_pipe<T, NS, MB, GK><<<grid, SPP_THREADS, SppRing<T, NS>::SMEM, ctx->stream>>>(    \
-        op->rowptr, op->colidx, (const T*)op->vals, (const T*)xsrc, (const T*)halo, n_loc,     \
-        (T*)y.ptr, op->rowblk, op->pblk, op->nblk, (T)a0, (T)a1, shifted ? 1 : 0,              \
-        (const T*)x.ptr, dotv ? (const T*)dotv->ptr : nullptr, op->part, ctx->d_sync, out, fz, ps)
-#define LAUNCH_V(T, NS, MB)                                                                    \
-    do {                                                                                       \
-        if (gk) LAUNCH_VG(T, NS, MB, true);                                                    \
-        else LAUNCH_VG(T, NS, MB, false);                                                      \
-    } while (0)
-        if (g_spmv_variant == 1) {
-            if (ctx->dtype == B2K_F64) LAUNCH_V(double, 2, 4);
-            else LAUNCH_V(float, 2, 4);
-        } else {
-            if (ctx->dtype == B2K_F64) LAUNCH_V(double, 3, 3);
-            else LAUNCH_V(float, 3, 3);
-        }
-#undef LAUNCH_V
-#undef LAUNCH_VG
+        b2k_dispatch(ctx, [&](auto t) {
+            using T = decltype(t);
+            b2k_flag(gk, [&](auto GK) {
+                b2k_flag(g_spmv_variant == 1, [&](auto v1) {      // variant 1: two stages of 4 row blocks, else 3 of 3
+                    constexpr int NS = v1 ? 2 : 3, MB = v1 ? 4 : 3;
+                    k_spmv_pipe<T, NS, MB, GK><<<grid, SPP_THREADS, SppRing<T, NS>::SMEM, ctx->stream>>>(
+                        op->rowptr, op->colidx, (const T*)op->vals, (const T*)xsrc, (const T*)halo, n_loc, (T*)y.ptr,
+                        op->rowblk, op->pblk, op->nblk, T(a0), T(a1), shifted ? 1 : 0, (const T*)x.ptr,
+                        dotv ? (const T*)dotv->ptr : nullptr, op->part, ctx->d_sync, out, fz, ps);
+                });
+            });
+        });
     } else {
         g_spmv_launch[0] = 1; g_spmv_launch[1] = 0; g_spmv_launch[2] = op->nblk; g_spmv_launch[3] = op->nblk;
-#define LAUNCH(T)                                                                              \
-    k_spmv_stream<T><<<op->nblk, SP_BT, 0, ctx->stream>>>(                                     \
-        op->rowptr, op->colidx, (const T*)op->vals, (const T*)xsrc, (const T*)halo, n_loc,     \
-        (T*)y.ptr, op->rowblk, (T)a0, (T)a1, shifted ? 1 : 0, (const T*)x.ptr,                 \
-        dotv ? (const T*)dotv->ptr : nullptr, op->part, ctx->d_sync, out, fz, ps)
-        if (ctx->dtype == B2K_F64) LAUNCH(double);
-        else LAUNCH(float);
-#undef LAUNCH
+        b2k_dispatch(ctx, [&](auto t) {
+            using T = decltype(t);
+            k_spmv_stream<T><<<op->nblk, SP_BT, 0, ctx->stream>>>(
+                op->rowptr, op->colidx, (const T*)op->vals, (const T*)xsrc, (const T*)halo, n_loc, (T*)y.ptr, op->rowblk,
+                T(a0), T(a1), shifted ? 1 : 0, (const T*)x.ptr, dotv ? (const T*)dotv->ptr : nullptr, op->part,
+                ctx->d_sync, out, fz, ps);
+        });
     }
     b2k_prof_end(ctx, pr);
     B2K_LAUNCH_CHECK(ctx);
@@ -2553,10 +2537,9 @@ extern "C" int32_t b2k_pencil_apply(b2k_ctx* ctx, const void* Pv, b2k_vec x, b2k
     }
     const double es = ctx->esize, n = (double)P->n;
     const double bytes = (double)P->A->nnz * (2 * es + 4) + 4.0 * (n + 1) + (has_prev ? 4.0 : 3.0) * es * n;
-    if (ctx->dtype == B2K_F64)
-        B2K_TRY((pencil_launch<double, 0>(ctx, P, r[0], r[1], r[2], rho, has_prev ? &r[3] : nullptr, beta, dot, bytes)));
-    else
-        B2K_TRY((pencil_launch<float, 0>(ctx, P, r[0], r[1], r[2], rho, has_prev ? &r[3] : nullptr, beta, dot, bytes)));
+    B2K_TRY(b2k_dispatch(ctx, [&](auto t) {
+        return pencil_launch<decltype(t), 0>(ctx, P, r[0], r[1], r[2], rho, has_prev ? &r[3] : nullptr, beta, dot, bytes);
+    }));
     if (!dot) return B2K_OK;
     B2K_TRY(b2k_fetch_results(ctx, 1, 0));
     *dot = ctx->h_res[0];
@@ -2587,10 +2570,9 @@ extern "C" int32_t b2k_pencil_rayleigh(b2k_ctx* ctx, const void* Pv, b2k_vec x, 
     }
     const double es = ctx->esize, n = (double)P->n;
     const double bytes = (double)P->A->nnz * (2 * es + 4) + 4.0 * (n + 1) + 3.0 * es * n;
-    if (ctx->dtype == B2K_F64)
-        B2K_TRY((pencil_launch<double, 1>(ctx, P, r[0], r[1], r[2], 0.0, nullptr, 0.0, want_dot, bytes)));
-    else
-        B2K_TRY((pencil_launch<float, 1>(ctx, P, r[0], r[1], r[2], 0.0, nullptr, 0.0, want_dot, bytes)));
+    B2K_TRY(b2k_dispatch(ctx, [&](auto t) {
+        return pencil_launch<decltype(t), 1>(ctx, P, r[0], r[1], r[2], 0.0, nullptr, 0.0, want_dot, bytes);
+    }));
     if (!want_dot) return B2K_OK;
     B2K_TRY(b2k_fetch_results(ctx, 2, 0));
     if (xax) *xax = ctx->h_res[0];
@@ -2719,8 +2701,7 @@ extern "C" int32_t b2k_op_apply_normal_gram(b2k_ctx* ctx, const b2k_op* op, b2k_
         return b2k_fail(ctx, B2K_ENOTSUP, "apply_normal_gram: more than %d columns", OP_ZMAX * OP_T);
     B2K_CUDA(ctx, cudaSetDevice(ctx->device));
     b2k_op* mop = const_cast<b2k_op*>(op);          // the per-CTA partial buffer is allocated on first use
-    if (ctx->dtype == B2K_F64) return onepass_t<double>(ctx, mop, rx, ry, rz);
-    return onepass_t<float>(ctx, mop, rx, ry, rz);
+    return b2k_dispatch(ctx, [&](auto t) { return onepass_t<decltype(t)>(ctx, mop, rx, ry, rz); });
 }
 
 // A/B switch of the one-pass dense step (tools / tests / bench.py's c4o child): 0 = variant A, 1 = variant B
@@ -2765,14 +2746,11 @@ extern "C" int32_t b2k_op_apply_block(b2k_ctx* ctx, const b2k_op* op, const b2k_
         for (int i = 0; i < SPM_PMAX; ++i) { cols.x[i] = ix[i0 + (i < np ? i : 0)]; cols.y[i] = iy[i0 + (i < np ? i : 0)]; }
         const int pr = b2k_prof_begin(ctx, 7, (double)op->nnz * (ctx->esize + 4) + 4.0 * (op->n_rows + 1) +
                                                   2.0 * np * ctx->esize * op->n_rows);
-        if (ctx->dtype == B2K_F64)
-            k_spmm_pipe<double><<<grid, SPP_THREADS, SpmRing<double>::SMEM, ctx->stream>>>(
-                op->rowptr, op->colidx, (const double*)op->vals, (double*)sp.base, sp.ld, cols, np, op->rowblk,
-                op->pblk, op->nblk);
-        else
-            k_spmm_pipe<float><<<grid, SPP_THREADS, SpmRing<float>::SMEM, ctx->stream>>>(
-                op->rowptr, op->colidx, (const float*)op->vals, (float*)sp.base, sp.ld, cols, np, op->rowblk,
-                op->pblk, op->nblk);
+        b2k_dispatch(ctx, [&](auto t) {
+            using T = decltype(t);
+            k_spmm_pipe<T><<<grid, SPP_THREADS, SpmRing<T>::SMEM, ctx->stream>>>(
+                op->rowptr, op->colidx, (const T*)op->vals, (T*)sp.base, sp.ld, cols, np, op->rowblk, op->pblk, op->nblk);
+        });
         b2k_prof_end(ctx, pr);
         B2K_LAUNCH_CHECK(ctx);
     }

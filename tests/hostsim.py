@@ -697,6 +697,11 @@ class HostSimLib:
         return L.OK
 
     def b2k_cg_chain(self, h, op, x, r, p, q, a0, a1, beta, rho, tol, nsteps, pq_out, normr_out, done):
+        hs = [int(v) for v in (x, r, p, q)]
+        for i in range(4):
+            for j in range(i):
+                if hs[i] == hs[j]:
+                    return self._fail(self._c(h), L.EINVAL, f"cg_chain: vectors {j} and {i} are the same")
         d = 0
         for i in range(nsteps):
             pq, nr = C.c_double(), C.c_double()
@@ -747,6 +752,11 @@ class HostSimLib:
 
     def b2k_bicgstab_chain(self, h, op, x, r, rs, p, v, s, t, a0, a1, rho, rho_old, alpha, omega, tol, nsteps,
                            rec_out, done):
+        hs = [int(w) for w in (x, r, rs, p, v, s, t)]
+        for i in range(7):
+            for j in range(i):
+                if hs[i] == hs[j]:
+                    return self._fail(self._c(h), L.EINVAL, f"bicgstab_chain: vectors {j} and {i} are the same")
         d = 0
         for i in range(nsteps):
             beta = (rho / rho_old) * (alpha / omega)

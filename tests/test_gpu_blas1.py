@@ -782,3 +782,26 @@ def test_bicgstab_chain_clamps_to_511(dt):
     assert got == want
     assert all(np.array_equal(w.to_host(), h) for w, h in zip(vs, chained))
     ctx.close()
+
+
+@pytest.mark.parametrize("dt", DTYPES, ids=["f64", "f32"])
+def test_cg_and_bicgstab_chains_refuse_aliased_vectors(dt):
+    """b2k_cg_chain with p == q and b2k_bicgstab_chain with p == v are refused (B2K_EINVAL) before anything is
+    enqueued: every vector keeps its bits."""
+    ctx, op, n = cg_setup(dt, coeffs=NONSYM)
+    hs, beta, rho = cg_state(ctx, n, dt, 4)
+    vs = [ctx.from_host(h) for h in hs]
+    x, r, p, _ = vs
+    pqs, nrs, done = (C.c_double * 4)(), (C.c_double * 4)(), C.c_int32()
+    assert ctx.lib.b2k_cg_chain(ctx.h, op.h, x.handle, r.handle, p.handle, p.handle, 0.0, 1.0, beta, rho, 0.0, 4, pqs,
+                                nrs, C.byref(done)) == L.EINVAL
+    assert all(np.array_equal(v.to_host(), h) for v, h in zip(vs, hs))
+    hs, scal = bicg_start(ctx, op, n, dt, 0.0, 1.0, 8)
+    vs = [ctx.from_host(h) for h in hs]
+    x, r, rs, p, _, s, t = vs
+    rec = np.zeros((4, 8))
+    assert ctx.lib.b2k_bicgstab_chain(ctx.h, op.h, x.handle, r.handle, rs.handle, p.handle, p.handle, s.handle, t.handle,
+                                      0.0, 1.0, *scal, 0.0, 4, rec.ctypes.data_as(C.POINTER(C.c_double)),
+                                      C.byref(done)) == L.EINVAL
+    assert all(np.array_equal(w.to_host(), h) for w, h in zip(vs, hs))
+    ctx.close()

@@ -250,6 +250,12 @@ def test_bicgstab_chain_bookkeeping(simf):
     G.test_bicgstab_chained_iterations_equal_stepwise()
 
 
+@pytest.mark.parametrize("dt", [np.float64, np.float32], ids=["f64", "f32"])
+def test_cg_and_bicgstab_chains_refuse_aliased_vectors(simf, dt):
+    import test_gpu_blas1 as B
+    B.test_cg_and_bicgstab_chains_refuse_aliased_vectors(dt)
+
+
 def test_basistransform_refusals(sim):
     """b2k_basis_transform's refusals (bad sizes, m > 256, two spaces, a repeated handle) leave every column as it
     was, on the simulator as on the device"""
